@@ -1,4 +1,4 @@
-"""bench.py — separated clips/sec of SAMAudio.separate() (10 s @ 48 kHz clips) on N B200s.
+"""bench.py — separated clips/sec of SAMAudio.separate() (10 s @ 48 kHz clips) on N H100s.
 
     python bench.py --gpus 1 --steps 3 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
@@ -7,6 +7,11 @@
 One "step" = one separate() over a batch of B synthetic clips per GPU (weak scaling): DAC-VAE encode,
 conditioning, 32 DiT evaluations (midpoint ODE), DAC-VAE decode of target+residual, and — for N>1 — the
 all-gather of the separated waveforms.  Prints ONE JSON line (rank 0).
+
+    python bench.py ... --dump-outputs DIR    # after the timed steps: DIR/target.npy, DIR/residual.npy (float32)
+
+With the same arguments the inputs (weights, clips, noise) are identical from run to run, so two builds can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -24,7 +29,7 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "separated clips/sec (10s@48kHz, sam-audio-large) at 1/2/4/8 B200 vs ref CPU"
+METRIC = "separated clips/sec (10s@48kHz, sam-audio-large) at 1/2/4/8 H100 vs ref CPU"
 UNIT = "clips/s"
 
 
@@ -34,7 +39,8 @@ def _peaks():
         d = json.load(open(p))
         return dict(hbm=float(d["hbm_gbs"]), tf_burst=float(d["bf16_tflops"]),
                     tf_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), source="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s — a bound, not a measured rate
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -275,7 +281,7 @@ def run_reference(args):
         "impl": "reference", "metric": METRIC, "value": v, "unit": UNIT, "n_gpus": args.gpus, "steps": len(vals),
         "warmup": n_warm, "ms_per_step": 1e3 / v, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
-        # the b200 arm's workload at this N (the driver pairs the two lines); the CPU leg times a bounded sample of it
+        # the GPU arm's workload at this N; the CPU leg times a bounded sample of it
         # (one clip of the batch, see cpu_baseline.sample): clips/s does not depend on which clip
         "config": _config(args, max(1, args.gpus), args.batch),
         "cpu_baseline": {"value": v, "unit": UNIT, "cores": cores, "cores_available": avail, "kind": "port",
@@ -300,7 +306,7 @@ def _config(args, world, batch):
         "model_shape": f"stand-in (HF config.json is gated): dim={tc.dim} layers={tc.n_layers} heads={tc.n_heads} "
                        f"ffn={tc.ffn_hidden}; DAC-VAE 64/1024/1536 rates 2-8-10-12; random-init weights",
         "global_batch": world * batch, "candidates": args.candidates, "clip_seconds": 10, "sample_rate": 48000,
-        "parallelism": f"dp{world}", "l2": "inputs_exceed_l2 (activations >> 126 MB)",
+        "parallelism": f"dp{world}", "l2": "inputs_exceed_l2 (activations >> 50 MB)",
         "text_encoder": "t5-base shape, random init, hash tokenizer (no checkpoint on disk)",
     }
 
@@ -308,6 +314,23 @@ def _config(args, world, batch):
 # ------------------------------------------------------------------------------------------------
 # GPU arm
 # ------------------------------------------------------------------------------------------------
+DUMP_CLIPS = 8     # 2 x 8 x 480000 fp32 = 31 MB
+
+
+def dump_outputs(out_dir, out):
+    """The waveforms separate() returned in the last timed step: a fixed, seeded sample of DUMP_CLIPS clips (all of
+    them when there are fewer), target and residual, as [k, samples] float32 arrays in clip order."""
+    import numpy as np
+    if isinstance(out, torch.Tensor):                 # N > 1: the all-gathered [clips, 2, samples]
+        target, residual = list(out[:, 0]), list(out[:, 1])
+    else:
+        target, residual = list(out.target), list(out.residual)
+    n = len(target)
+    pick = sorted(torch.randperm(n, generator=torch.Generator().manual_seed(0))[:DUMP_CLIPS].tolist())
+    os.makedirs(out_dir, exist_ok=True)
+    for name, wavs in (("target", target), ("residual", residual)):
+        arr = torch.stack([wavs[i].detach().float().cpu() for i in pick]).numpy()
+        np.save(os.path.join(out_dir, f"{name}.npy"), arr.astype(np.float32))
 def run_gpu(args):
     import __graft_entry__ as g
     world, rank, local = _dist_setup(args.gpus)
@@ -420,11 +443,17 @@ def run_gpu(args):
     sampler = ClockSampler(local) if rank == 0 else None
     # ---- value: inputs resident in HBM (the ODE solve replays as one CUDA graph) ----
     eng.launch_count(reset=True)
-    ms_val = timed(lambda: step_resident(batch_gpu, noise_gpu), args.steps)
+    last = {}
+    ms_val = timed(lambda: last.__setitem__("out", step_resident(batch_gpu, noise_gpu)), args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
+    del last
     launches = eng.launch_count(reset=True)
-    # ---- the same K steps again with one CUDA event in front of every launch: live per-kernel times ----
+    # ---- one more step with a CUDA event in front of every launch: live per-kernel times.  Every step replays the same
+    #      captured graph, so one step gives the per-step breakdown; K more would only lengthen the run ----
+    prof_steps = 1
     eng.profile(True)
-    ms_prof = timed(lambda: step_resident(batch_gpu, noise_gpu), args.steps)
+    ms_prof = timed(lambda: step_resident(batch_gpu, noise_gpu), prof_steps)
     prof = eng.profile_report()
     eng.profile(False)
     eng.launch_count(reset=True)
@@ -442,8 +471,8 @@ def run_gpu(args):
     clips_total = world * B * args.steps
     value = clips_total / (ms_val / 1e3)
     e2e = clips_total / (ms_e2e / 1e3)
-    # dominant kernel = the tcgen05 GEMM (all DiT linears + codec convs): aggregate its launches
-    # tensor-bound launches of the tcgen05 GEMM: algorithmic intensity above the ridge (peak FLOP/s / HBM bytes/s); the
+    # dominant kernel = the wgmma GEMM (all DiT linears + codec convs): aggregate its launches
+    # tensor-bound launches of the wgmma GEMM: algorithmic intensity above the ridge (peak FLOP/s / HBM bytes/s); the
     # weight-streaming launches below it (per-item bias GEMMs, text K/V, time embedders, 48 kHz codec stages) are
     # HBM-bound and reported under hbm_kernels instead
     ridge = peaks["tf_sustained"] * 1e12 / (peaks["hbm"] * 1e9)
@@ -468,16 +497,12 @@ def run_gpu(args):
             groups["norm_elementwise"] += v["ms"]
     # HBM-bound kernels: algorithmic bytes per launch / live launch time vs the measured copy bandwidth
     hbm_tags = [t for t in prof if prof[t]["bytes"] > 0 and t not in gemm_tags]
-    hbm = {t: {"launches_per_step": prof[t]["launches"] / args.steps,
+    hbm = {t: {"launches_per_step": prof[t]["launches"] / prof_steps,
                "mb_per_launch": round(prof[t]["bytes"] / prof[t]["launches"] / 1e6, 2),
-               "ms_per_step": round(prof[t]["ms"] / args.steps, 3),
+               "ms_per_step": round(prof[t]["ms"] / prof_steps, 3),
                "gbs": round(prof[t]["bytes"] / max(prof[t]["ms"], 1e-9) / 1e6, 1),
                "frac": round(prof[t]["bytes"] / max(prof[t]["ms"], 1e-9) / 1e6 / peaks["hbm"], 3)}
            for t in sorted(hbm_tags, key=lambda t: -prof[t]["ms"])}
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "roofline_traffic_r2.json")
-    if os.path.exists(tpath):     # dram__bytes_read+write of the dominant launch (ffn.w13) from the committed ncu capture
-        traffic = json.load(open(tpath))
     att = {t: v for t, v in prof.items() if t.startswith("sdpa")}
     att_tf = sum(v["flops"] for v in att.values()) / max(sum(v["ms"] for v in att.values()), 1e-9) / 1e9
     line = {
@@ -489,30 +514,26 @@ def run_gpu(args):
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": int(launches),
         "clocks": clocks,
-        "roofline": {"kernel": "gemm_tc_kernel (tcgen05 segmented GEMM: launches above the roofline ridge = DiT linears "
+        "roofline": {"kernel": "gemm_tc_kernel (wgmma segmented GEMM: launches above the roofline ridge = DiT linears "
                                "+ the wide codec convs)",
                      "bound": "tensor", "achieved": achieved, "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
                      "frac": achieved / peaks["tf_sustained"],
-                     "traffic": None if traffic is None else traffic["traffic_bytes_per_launch"],
-                     "traffic_note": None if traffic is None else
-                     f"{traffic['kernel']}: dram read+write per launch from ncu --set full "
-                     f"(algorithmic {traffic['algorithmic_bytes_per_launch']} B); {traffic['source']}",
-                     "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peaks['source']})",
+                     "peak_source": peaks["source"],
                      "launches": int(g_n), "avg_launch_ms": g_ms / max(g_n, 1),
                      "share_of_step": g_ms / max(total_ms, 1e-9),
-                     "profiled_ms_per_step": ms_prof / args.steps,
-                     "algorithmic_tflop_per_step": g_fl / 1e12 / args.steps,
+                     "profiled_ms_per_step": ms_prof / prof_steps,
+                     "algorithmic_tflop_per_step": g_fl / 1e12 / prof_steps,
                      "dominant_launch": (lambda t: {"tag": t, "launches": int(prof[t]["launches"]),
                                                     "avg_launch_ms": prof[t]["ms"] / max(prof[t]["launches"], 1),
                                                     "tflop_per_launch": prof[t]["flops"] / max(prof[t]["launches"], 1) / 1e12,
                                                     "achieved": prof[t]["flops"] / max(prof[t]["ms"], 1e-9) / 1e9,
                                                     "frac": prof[t]["flops"] / max(prof[t]["ms"], 1e-9) / 1e9 / peaks["tf_sustained"]})(
                          max(gemm_tags, key=lambda t: prof[t]["ms"])) if gemm_tags else None},
-        "breakdown_ms_per_step": {k: v / args.steps for k, v in groups.items()},
+        "breakdown_ms_per_step": {k: v / prof_steps for k, v in groups.items()},
         "hbm_kernels": {"peak_gbs": peaks["hbm"], "note": "algorithmic bytes (operands once + every epilogue stream "
                         "once) / live launch time, sustained inside the step", "kernels": hbm},
         "sdpa_tflops": att_tf,
-        "kernels": {t: {"ms_per_step": round(v["ms"] / args.steps, 3), "launches_per_step": v["launches"] / args.steps,
+        "kernels": {t: {"ms_per_step": round(v["ms"] / prof_steps, 3), "launches_per_step": v["launches"] / prof_steps,
                         "tflops": round(v["flops"] / max(v["ms"], 1e-9) / 1e9, 1)}
                     for t, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"])},
         "workspace_gib": eng.workspace_bytes() / 2 ** 30,
@@ -545,7 +566,7 @@ if __name__ == "__main__":
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="cuda", choices=["cuda", "reference"])
     ap.add_argument("--model", default="sam-audio-large")
     ap.add_argument("--batch", type=int, default=64, help="clips per GPU per step")
     ap.add_argument("--candidates", type=int, default=1, help="reranking_candidates (BASELINE config 4: 8)")
@@ -554,6 +575,9 @@ if __name__ == "__main__":
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--gather", default="overlap", choices=["overlap", "after"],
                     help="N>1: all-gather each decoded chunk under the next chunk's decode, or once after the decode")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the separated waveforms of the last timed step (a fixed sample "
+                         f"of at most {DUMP_CLIPS} clips) as DIR/target.npy and DIR/residual.npy, float32")
     a = ap.parse_args()
     if a.impl == "reference":
         run_reference(a)

@@ -1,4 +1,4 @@
-/* samaudio_b200.h — C ABI of libsamaudio_b200.so: the B200 (sm_100a) implementation of the
+/* samaudio_b200.h — C ABI of libsamaudio_b200.so: the H100 (sm_90a) implementation of the
  * SAMAudio.separate() inference hot path of facebookresearch/sam-audio.
  *
  * The reference has no FFI: its seam is the Python class surface (SURVEY.md §8b).  Each entry point
@@ -147,23 +147,20 @@ int sab_t5_forward(sab_t5* e, const int64_t* ids, const uint8_t* mask, const int
 int64_t sab_t5_launch_count(sab_t5* e, int reset);
 
 /* ---- unit-test seams (used by tests/ only; stable but not part of the drop-in surface) ---- */
-/* C[M,N] (fp32) = A[M,K] (bf16) * B[N,K]^T (bf16) through the tcgen05 GEMM (tile BN x BK; cg = 1: one CTA per
- * 128-row tile, cg = 2: cta_group::2 pairs on 256-row tiles, cg = 0: the engine's default choice). */
+/* C[M,N] (fp32) = A[M,K] (bf16) * B[N,K]^T (bf16) through the wgmma GEMM (tile BN x BK; cg = 1: one CTA per
+ * 128-row tile, cg = 2: 2-CTA clusters on 256-row tiles sharing the B tile, cg = 0: the engine's default choice). */
 int sab_test_gemm(int M, int N, int K, const void* a_bf16, const void* b_bf16, float* c, int bn, int bk, int cg,
                   void* stream);
 /* O = softmax(Q K^T / sqrt(128) + mask) V through the attention kernel; all [items*T, heads*128] bf16. */
 int sab_test_attention(int items, int heads, int Tq, int Tk, const void* q, const void* k, const void* v,
                        const uint8_t* key_mask, void* o, void* stream);
 
-/* Same, through the tcgen05 self-attention kernel (Tq == Tk == T <= 256); v_lbo / v_sbo <= 0 select the
- * defaults of the MN-major V descriptor. */
-int sab_test_attention_tc(int items, int heads, int T, const void* q, const void* k, const void* v,
-                          const uint8_t* key_mask, void* o, int v_lbo, int v_sbo, void* stream);
-/* second-generation kernel (attention_tc2.cuh): shift_log2 >= 0 = single-pass softmax with that logit bound,
- * < 0 = exact two-pass; poly = pairs of every 8 exponentials evaluated on the FMA pipe (0..4, < 0: default);
- * trace: null, or a device buffer of 8 x 32 x 8 int64 that CTA 0 fills with clock64() stamps (tools/attn_trace.py). */
+/* Same, through the wgmma self-attention kernel (attention_tc2.cuh; Tq == Tk == T <= 256): shift_log2 > 0 =
+ * single-pass softmax with that logit bound, < 0 = exact two-pass, 0 = the folded variant (q already scaled by
+ * log2(e)/sqrt(128), logits bounded by 50); poly = pairs of every 8 exponentials evaluated on the FMA pipe
+ * (0, 2, 3, 4; < 0: default). */
 int sab_test_attention_tc2(int items, int heads, int T, const void* q_bf16, const void* k_bf16, const void* v_bf16,
-                           const uint8_t* key_mask, void* o_bf16, float shift_log2, int poly, long long* trace, void* stream);
+                           const uint8_t* key_mask, void* o_bf16, float shift_log2, int poly, void* stream);
 
 /* Visual prompting, frame pre-processing.  replaces: PerceptionEncoder.get_transform (vision_encoder.py:91-113) =
  * torchvision Resize((S, S), BICUBIC, antialias) on uint8 frames, x / 255, Normalize(0.5, 0.5).

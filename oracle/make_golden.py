@@ -199,9 +199,11 @@ def main():
         print(f"SAMAudio.forward[{tag}] restatement vs reference: rel_l2={e:.3e}")
         assert e < 2e-5, e
         outs[tag] = r
+    # inputs and outputs in two files (tests/_util.py load_golden merges them): each fixture file stays under 1 MB
     torch.save(dict(noisy=noisy, feats=feats, text=text, video=video, time=time, text_mask=mem_mask,
-                    anchor_ids=ids, anchor_alignment=al, pad_mask=pad_mask, out=outs),
+                    anchor_ids=ids, anchor_alignment=al, pad_mask=pad_mask),
                os.path.join(GOLDEN, "samaudio_forward_tiny.pt"))
+    torch.save(dict(out=outs), os.path.join(GOLDEN, "samaudio_forward_tiny.1.pt"))
 
     # ---------------- visual prompting: PerceptionEncoder transform + chunked encode (reference classes) ----------------
     from sam_audio.model import vision_encoder as ref_ve
@@ -262,7 +264,9 @@ def main():
     model.text_ranker = None
     sep["ranked3"] = dict(target=[t.clone() for t in r.target], residual=[t.clone() for t in r.residual], noise=noise,
                           scores=_FixedRanker.SCORES.clone())
-    torch.save(dict(lens=lens2, results=sep), os.path.join(GOLDEN, "separate_tiny.pt"))
+    torch.save(dict(lens=lens2, results={1: sep[1], 2: sep[2]}), os.path.join(GOLDEN, "separate_tiny.pt"))
+    torch.save(dict(results={8: sep[8]}), os.path.join(GOLDEN, "separate_tiny.1.pt"))
+    torch.save(dict(results={"ranked3": sep["ranked3"]}), os.path.join(GOLDEN, "separate_tiny.2.pt"))
     for f in sorted(os.listdir(GOLDEN)):
         print(f, os.path.getsize(os.path.join(GOLDEN, f)))
 

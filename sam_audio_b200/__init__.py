@@ -1,4 +1,4 @@
-"""sam_audio_b200 — B200-native (sm_100a) implementation of the SAMAudio.separate() hot path.
+"""sam_audio_b200 — H100-native (sm_90a) implementation of the SAMAudio.separate() hot path.
 
 Public surface mirrors the reference package (reference: sam_audio/__init__.py:3-4):
 ``SAMAudio``, ``SAMAudioProcessor`` (+ ``Batch``, ``SeparationResult``).

@@ -39,7 +39,7 @@ class SabT5Config(ctypes.Structure):
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
-    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_attention", "sab_test_attention_tc", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_attention", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -55,7 +55,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(path):
             raise RuntimeError(
                 f"{_LIB_NAME} not built ({path}); run `python -c 'import __graft_entry__ as g; g.build()'`. "
-                "The B200 separation path has no CPU/PyTorch fallback.")
+                "The H100 separation path has no CPU/PyTorch fallback.")
         L = ctypes.CDLL(path)
         vp, i32, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
         L.sab_last_error.restype = ctypes.c_char_p
@@ -76,8 +76,7 @@ def lib() -> ctypes.CDLL:
         L.sab_profile_report.argtypes = [vp, ctypes.c_char_p, i64, vp]
         L.sab_test_gemm.argtypes = [i32, i32, i32, vp, vp, vp, i32, i32, i32, vp]
         L.sab_test_attention.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
-        L.sab_test_attention_tc.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp]
-        L.sab_test_attention_tc2.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp, vp]
+        L.sab_test_attention_tc2.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp]
         L.sab_preprocess_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
         L.sab_test_aa_taps.argtypes = [i32, i32, i32, vp, vp, vp, vp]
         L.sab_test_solver_grid.argtypes = [i32, i32, i32, vp, vp]

@@ -1,4 +1,4 @@
-"""Configuration objects for the B200 SAM-Audio separation path.
+"""Configuration objects for the H100 SAM-Audio separation path.
 
 Mirrors the JSON schema of the reference's ``config.json``
 (reference: sam_audio/model/config.py:10-41 DACVAEConfig, :49-61 T5EncoderConfig,

@@ -1,47 +1,34 @@
-// tcgen05 self-attention, second generation, for sequences of up to 256 keys (10 s clips: T = 250), head_dim = 128.
+// wgmma self-attention for sequences of up to 256 keys (10 s clips: T = 250), head_dim = 128.
 // reference: sam_audio/model/transformer.py:153-160 (SDPA, scale 1/sqrt(hd), bool key mask, True = attend).
 //
-// What bounded the first kernel (attention_tc.cuh; 22.5 % tensor pipe, ncu): the softmax read S twice out of TMEM
-// (64 B/clk per SM sub-partition), ran on 8 warps with every exponential on the MUFU pipe (16/clk/SM: 4096 clk per
-// (item, head), as long as all four MMAs together), and each thread stored its own output row (a 16-byte store per
-// lane to 32 different lines: ~66 L1 wavefront-clk per instruction, ~8 k clk per work item).  Here:
-//   * 19 warps: MMA issuer, TMA loader, TMA storer, and 2 x 8 softmax warps — one group of 8 per 128-query tile, two
-//     warps per TMEM lane quarter, each owning half of the key columns (thread = query row x key half);
-//   * ONE pass over S: with QK-RMSNorm (transformer.py:117-119,145-148) |q.k|/sqrt(hd) <= sqrt(hd) max|w_q| max|w_k|, so
-//     a per-layer constant `shift` >= every logit replaces the row maximum (softmax is shift-invariant; the engine
-//     picks this variant only while 2 x shift stays far inside the fp32 exponent range, else the exact
-//     two-pass variant `kExact`, which is also what the raw-q/k test seam uses);
-//   * a quarter to a half of the exponentials (template kPoly) run on the FMA pipe: Cody-Waite range reduction +
-//     degree-3 minimax polynomial in packed f32x2 arithmetic (rel. error 7.5e-5, far below bf16's 3.9e-3);
-//   * P is written back to TMEM in place as the A operand of the second MMA: the low key half ascending from column 0,
-//     the high key half (processed in descending chunk order) descending from column 256, which leaves the middle
-//     128 columns free for O (one N = 128 MMA per key step: with N = 64 the TMEM read of the A operand, 4 KB per
-//     instruction, bounds the MMA at half rate — measured), so a tile owns 256 TMEM columns from QK^T to its
-//     epilogue and both tiles of an (item, head) are in flight against one issuing thread;
-//   * in the engine the softmax scale log2(e)/sqrt(hd) is folded into the q-norm weights by the QKV epilogue and the
-//     logit bound is small enough (<= 50) that no shift is needed at all: p = 2^s straight from the accumulator
-//     (template kFolded), one instruction less per element on an issue-bound loop;
-//   * the epilogue scales by 1/rowsum, writes bf16 rows into a 128B-swizzled shared-memory tile and a dedicated warp
-//     TMA-stores it (rows past the sequence end are clipped by the tensor map).
-//
-//   TMEM (per tile m, base 256 m):  S = [0,256);  then P keys 0..127 in [0,64), P keys 128..255 in [192,256),
-//                                   O (128 dims) in [64,192)
+// One CTA per (item, head): TMA brings Q (one or two 128-query tiles), K and V ([256 x 128] each, SWIZZLE_128B,
+// zero-filled past the sequence end) into shared memory once; two consumer warpgroups own 64 query rows each and
+// walk the query tiles.  Everything between the two HBM touches stays on chip, the scores in registers:
+//   wgmma : S = Q K^T            (m64n256k16 x 8, both operands from shared memory) -> 128 fp32 registers / thread
+//   CUDA  : row softmax on the accumulator fragment (a row lives in the 4 lanes of a quad)
+//   wgmma : O = P V              (m64n128k16 x 16, A = P as bf16 register fragments, B = V MN-major smem)
+//   CUDA  : O / rowsum -> bf16 -> global, head-major "(h d)"
+// Softmax variants: exact (two-pass row maximum), single pass with a per-layer bound `shift` >= every logit (with
+// QK-RMSNorm, transformer.py:117-119,145-148: |q.k|/sqrt(hd) <= sqrt(hd) max|w_q| max|w_k|; softmax is
+// shift-invariant), and `folded`, where the engine's QKV epilogue has already scaled q into the log2 domain and the
+// bound is small enough (<= 50) that p = 2^s needs neither scale nor shift.  kPoly of every 8 exponential pairs run
+// on the FMA pipe (Cody-Waite range reduction + degree-3 minimax polynomial, rel. error 7.5e-5, far below bf16's
+// 3.9e-3), the rest on the MUFU.
+// Longer sequences use the streaming kernel in attention.cuh.
 #pragma once
 #include "common.cuh"
-#include "attention_tc.cuh"
+#include "wgmma.cuh"
 
 namespace sab {
 
-constexpr int AT2_THREADS = 19 * 32;              // warps 0/1/2: MMA issue + TMEM alloc, TMA load, TMA store; 3..18: softmax
+constexpr int AT2_THREADS = 256;                  // two consumer warpgroups
 constexpr int AT2_Q_BYTES = 128 * 128 * 2;        // 32 KB per 128-query tile (2 boxes of [128 x 64])
 constexpr int AT2_KV_BYTES = 256 * 128 * 2;       // 64 KB (2 boxes of [256 x 64])
-constexpr int AT2_O_BYTES = 128 * 128 * 2;        // 32 KB output staging tile (2 boxes of [128 x 64])
-constexpr int AT2_BAR_BYTES = 256;
-constexpr int AT2_XCH_BYTES = 2 * 2 * 128 * 4;    // row sums (and, exact variant, row maxima) exchanged between key halves
-constexpr int AT2_SMEM = 2 * AT2_Q_BYTES + 2 * AT2_KV_BYTES + AT2_O_BYTES + AT2_BAR_BYTES + AT2_XCH_BYTES;
+constexpr int AT2_SMEM = 2 * AT2_Q_BYTES + 2 * AT2_KV_BYTES + 256 /*key validity*/ + 64 /*barriers*/ + 1024 /*alignment*/;
 static_assert(AT2_SMEM <= 227 * 1024, "attention_tc2: shared memory budget");
 
 struct AttnTc2Params {
+  __nv_bfloat16* o; long long o_ld; // output [items * T, o_ld], head h at columns [128h, 128h + 128)
   const uint8_t* key_mask;          // [items / mask_div, Tk] or null
   int T, heads, items;
   int mask_div;                     // mask row = item / mask_div (candidates share their clip's pad mask); 0/1: item
@@ -49,381 +36,171 @@ struct AttnTc2Params {
   float scale_log2;                 // log2(e) / sqrt(hd)
   float shift_log2;                 // single-pass variant: a bound on every scaled logit (log2 domain)
   int reverse;                      // walk the items from the last to the first (serpentine L2 reuse, engine.cu)
-  long long* trace;                 // debug timeline (tools/attn_trace.py): CTA 0 stamps clock64() at its hand-over
-                                    // points, [item < AT2_TRACE_ITEMS][warp][8 events]; null in production
 };
-constexpr int AT2_TRACE_ITEMS = 8;
-SAB_DEVICE void at2_stamp(long long* trace, int j, int warp, int ev) {
-  if (trace != nullptr && blockIdx.x == 0 && j < AT2_TRACE_ITEMS) trace[(j * 32 + warp) * 8 + ev] = clock64();
-}
 
-SAB_DEVICE void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
+SAB_DEVICE float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
 }
-SAB_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-SAB_DEVICE void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-SAB_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-template <int kId>
-SAB_DEVICE void named_bar_sync256() { asm volatile("bar.sync %0, 256;" ::"n"(kId) : "memory"); }
-SAB_DEVICE void group_sync(int m) { if (m == 0) named_bar_sync256<1>(); else named_bar_sync256<2>(); }
-
-// ---- packed f32x2 arithmetic (FFMA2 / FADD2: two lanes of fp32 per instruction) ----
-SAB_DEVICE uint64_t f2_pack(float a, float b) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-SAB_DEVICE void f2_unpack(uint64_t r, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(r)); }
-SAB_DEVICE uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.ftz.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-SAB_DEVICE uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.ftz.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-SAB_DEVICE uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.ftz.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// 2^x for x <= 0 on the FMA / ALU pipes: n = rint(x), f = x - n in [-1/2, 1/2], 2^f by a degree-3 minimax polynomial
-// (relative error 7.5e-5), 2^n by adding n to the exponent field.  Two values per call (packed arithmetic).
-SAB_DEVICE void exp2_poly2(float x0, float x1, float& p0, float& p1) {
+// 2^x on the FMA / ALU pipes: n = rint(x), f = x - n in [-1/2, 1/2], 2^f by a degree-3 minimax polynomial
+// (relative error 7.5e-5), 2^n by adding n to the exponent field
+SAB_DEVICE float exp2_poly(float x) {
   constexpr float kMagic = 12582912.f;   // 1.5 * 2^23: adding it rounds to the nearest integer
-  x0 = fmaxf(x0, -125.f);
-  x1 = fmaxf(x1, -125.f);
-  const uint64_t x = f2_pack(x0, x1);
-  const uint64_t t = f2_add(x, f2_pack(kMagic, kMagic));
-  const uint64_t n = f2_add(t, f2_pack(-kMagic, -kMagic));
-  const uint64_t f = f2_fma(n, f2_pack(-1.f, -1.f), x);
-  uint64_t p = f2_fma(f2_pack(0.0551716648f, 0.0551716648f), f, f2_pack(0.2426111251f, 0.2426111251f));
-  p = f2_fma(p, f, f2_pack(0.6932609677f, 0.6932609677f));
-  p = f2_fma(p, f, f2_pack(0.9999280572f, 0.9999280572f));
-  float t0, t1, q0, q1;
-  f2_unpack(t, t0, t1);
-  f2_unpack(p, q0, q1);
-  p0 = __int_as_float(__float_as_int(q0) + (__float_as_int(t0) << 23));
-  p1 = __int_as_float(__float_as_int(q1) + (__float_as_int(t1) << 23));
+  x = fmaxf(x, -125.f);
+  const float t = __fadd_rn(x, kMagic);
+  const float n = __fadd_rn(t, -kMagic);
+  const float f = __fadd_rn(x, -n);
+  float p = fmaf(0.0551716648f, f, 0.2426111251f);
+  p = fmaf(p, f, 0.6932609677f);
+  p = fmaf(p, f, 0.9999280572f);
+  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
-
-// 2^x for |x| <= 50 (no clamp): the folded single-pass path, where the engine guarantees the logit bound
-SAB_DEVICE void exp2_poly2_small(uint64_t x, float& p0, float& p1) {
-  constexpr float kMagic = 12582912.f;
-  const uint64_t t = f2_add(x, f2_pack(kMagic, kMagic));
-  const uint64_t n = f2_add(t, f2_pack(-kMagic, -kMagic));
-  const uint64_t f = f2_fma(n, f2_pack(-1.f, -1.f), x);
-  uint64_t p = f2_fma(f2_pack(0.0551716648f, 0.0551716648f), f, f2_pack(0.2426111251f, 0.2426111251f));
-  p = f2_fma(p, f, f2_pack(0.6932609677f, 0.6932609677f));
-  p = f2_fma(p, f, f2_pack(0.9999280572f, 0.9999280572f));
-  float t0, t1, q0, q1;
-  f2_unpack(t, t0, t1);
-  f2_unpack(p, q0, q1);
-  p0 = __int_as_float(__float_as_int(q0) + (__float_as_int(t0) << 23));
-  p1 = __int_as_float(__float_as_int(q1) + (__float_as_int(t1) << 23));
-}
-
-// one chunk of 32 scores of this thread's row -> 32 probabilities (16 packed bf16 pairs), row-sum accumulated.
-// kFolded: the scores are already in the log2 domain and bounded by +-50 (p = 2^s, no scale, no shift).
-template <int kPoly, bool kMasked, bool kFolded>
-SAB_DEVICE void softmax_chunk_impl(const float (&v)[32], uint32_t bits, float scale, float nshift, uint64_t& sum2,
-                                   uint32_t (&pk)[16]) {
-  const uint64_t sc2 = f2_pack(scale, scale), sh2 = f2_pack(nshift, nshift);
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    float x0 = v[2 * j], x1 = v[2 * j + 1], p0, p1;
-    if (!kFolded) f2_unpack(f2_fma(f2_pack(x0, x1), sc2, sh2), x0, x1);
-    if ((j & 7) < kPoly) {          // kPoly of every 8 pairs on the FMA pipe, the rest on the MUFU
-      if (kFolded) exp2_poly2_small(f2_pack(x0, x1), p0, p1);
-      else exp2_poly2(x0, x1, p0, p1);
-    } else {
-      p0 = ex2_approx(x0);
-      p1 = ex2_approx(x1);
-    }
-    if (kMasked) {
-      p0 = ((bits >> (2 * j)) & 1u) ? p0 : 0.f;
-      p1 = ((bits >> (2 * j + 1)) & 1u) ? p1 : 0.f;
-    }
-    sum2 = f2_add(sum2, f2_pack(p0, p1));
-    pk[j] = pack_bf16(p0, p1);
-  }
-}
-// all 32 keys valid (every chunk but the sequence's last): no per-element predication in the hot path
-template <int kPoly, bool kFolded>
-SAB_DEVICE void softmax_chunk(const float (&v)[32], uint32_t bits, float scale, float nshift, uint64_t& sum2,
-                              uint32_t (&pk)[16]) {
-  if (bits == 0xffffffffu) softmax_chunk_impl<kPoly, false, kFolded>(v, bits, scale, nshift, sum2, pk);
-  else softmax_chunk_impl<kPoly, true, kFolded>(v, bits, scale, nshift, sum2, pk);
-}
-
 template <bool kExact, int kPoly, bool kFolded>
 __global__ void __launch_bounds__(AT2_THREADS, 1)
 attention_tc2_kernel(const __grid_constant__ CUtensorMap tm_q /*box 64 x 128*/,
                      const __grid_constant__ CUtensorMap tm_k /*box 64 x 256*/,
                      const __grid_constant__ CUtensorMap tm_v /*box 64 x 256*/,
-                     const __grid_constant__ CUtensorMap tm_o /*box 64 x 128, output [items, T, heads*128]*/,
                      const __grid_constant__ AttnTc2Params P) {
-  extern __shared__ __align__(1024) uint8_t at2_smem[];
+  extern __shared__ uint8_t at2_raw[];
+  uint8_t* at2_smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at2_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = at2_smem;                          // two query tiles
   uint8_t* sK = sQ + 2 * AT2_Q_BYTES;
   uint8_t* sV = sK + AT2_KV_BYTES;
-  uint8_t* sO = sV + AT2_KV_BYTES;                 // output staging (shared by both tiles, used alternately)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sO + AT2_O_BYTES);
+  uint8_t* s_valid = sV + AT2_KV_BYTES;            // [256] key < T and not masked
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_valid + 256);
   uint64_t *bar_qk0 = bars, *bar_q1 = bars + 1, *bar_v = bars + 2;
-  uint64_t *bar_s = bars + 3 /*[2]*/, *bar_p = bars + 5 /*[2]*/, *bar_o = bars + 7 /*[2]*/, *bar_e = bars + 9 /*[2]*/;
-  uint64_t *bar_full = bars + 11 /*[2]*/, *bar_free = bars + 13;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
-  float* xch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + AT2_BAR_BYTES);   // [tile][half][row]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;                        // consumer warpgroup: query rows 64 wg .. 64 wg + 63 of a tile
   const int n_mt = (P.T + 127) / 128;              // 1 or 2 query tiles
-  const int n_work = P.heads * P.items;            // persistent CTAs loop over (item, head)
+  const int w = blockIdx.x;
+  const int head = w % P.heads, item = P.reverse ? P.items - 1 - w / P.heads : w / P.heads;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      if (smem_u32(at2_smem) & 1023u) __trap();    // SWIZZLE_128B operands need 1 KB alignment (no slack is reserved)
-      tma_prefetch_desc(&tm_q);
-      tma_prefetch_desc(&tm_k);
-      tma_prefetch_desc(&tm_v);
-      tma_prefetch_desc(&tm_o);
-      mbar_init(bar_qk0, 1);
-      mbar_init(bar_q1, 1);
-      mbar_init(bar_v, 1);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(bar_s + i, 1);
-        mbar_init(bar_p + i, 8);       // one arrive per softmax warp of the tile's group
-        mbar_init(bar_o + i, 1);
-        mbar_init(bar_e + i, 8);
-        mbar_init(bar_full + i, 8);
-      }
-      mbar_init(bar_free, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<512>(tmem_slot);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_q);
+    tma_prefetch_desc(&tm_k);
+    tma_prefetch_desc(&tm_v);
+    mbar_init(bar_qk0, 1);
+    mbar_init(bar_q1, 1);
+    mbar_init(bar_v, 1);
+    fence_barrier_init();
   }
-  tc_fence_before();
+  {
+    const uint8_t* mk = P.key_mask ? P.key_mask + (long long)(P.mask_div > 1 ? item / P.mask_div : item) * P.T : nullptr;
+    const int key = threadIdx.x;
+    s_valid[key] = (key < P.T && (!mk || mk[key])) ? 1 : 0;
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  if (threadIdx.x == 0) {
+    const int qc = P.q_col0 + head * 128, kc = P.k_col0 + head * 128, vc = P.v_col0 + head * 128;
+    mbar_expect_tx(bar_qk0, AT2_Q_BYTES + AT2_KV_BYTES);
+    tma_load_3d(sQ, &tm_q, bar_qk0, qc, 0, item);
+    tma_load_3d(sQ + AT2_Q_BYTES / 2, &tm_q, bar_qk0, qc + 64, 0, item);
+    tma_load_3d(sK, &tm_k, bar_qk0, kc, 0, item);
+    tma_load_3d(sK + AT2_KV_BYTES / 2, &tm_k, bar_qk0, kc + 64, 0, item);
+    if (n_mt > 1) {
+      mbar_expect_tx(bar_q1, AT2_Q_BYTES);
+      tma_load_3d(sQ + AT2_Q_BYTES, &tm_q, bar_q1, qc, 128, item);
+      tma_load_3d(sQ + AT2_Q_BYTES + AT2_Q_BYTES / 2, &tm_q, bar_q1, qc + 64, 128, item);
+    }
+    mbar_expect_tx(bar_v, AT2_KV_BYTES);
+    tma_load_3d(sV, &tm_v, bar_v, vc, 0, item);
+    tma_load_3d(sV + AT2_KV_BYTES / 2, &tm_v, bar_v, vc + 64, 0, item);
+  }
 
-  if (warp == 0) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 256);
-      constexpr uint32_t idesc_o = make_idesc_bf16_bmn(128, 128);
-      int j = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++j) {
-        const uint32_t ph = j & 1;
-        // ---- S_m = Q_m K^T -> TMEM cols [256m, 256m + 256); the tile's columns are free once the previous item's
-        //      epilogue has read its O out of them ----
-        for (int m = 0; m < n_mt; ++m) {
-          if (j > 0) mbar_wait(bar_e + m, ph ^ 1);
-          at2_stamp(P.trace, j, 0, 2 * m);           // S columns free
-          mbar_wait(m == 0 ? bar_qk0 : bar_q1, ph);
-          at2_stamp(P.trace, j, 0, 2 * m + 1);       // operands landed: QK^T issued
-          tc_fence_after();
+  // accumulator fragment: this thread holds rows r0 and r0 + 8 of the warpgroup's 64, columns 8i + 2 (lane % 4) + {0, 1}
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  const float scale = kFolded ? 1.f : P.scale_log2;
+  for (int m = 0; m < n_mt; ++m) {
+    mbar_wait(m == 0 ? bar_qk0 : bar_q1, 0);
+    // ---- S = Q K^T ----
+    float s[128];
 #pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            const uint32_t qa = smem_u32(sQ) + m * AT2_Q_BYTES + (ks >> 2) * (AT2_Q_BYTES / 2);
-            const uint32_t ka = smem_u32(sK) + (ks >> 2) * (AT2_KV_BYTES / 2);
-            umma_f16(tmem + m * 256, make_kmajor_desc<128>(qa) + (uint64_t)((ks & 3) * 2),
-                     make_kmajor_desc<128>(ka) + (uint64_t)((ks & 3) * 2), idesc_s, ks ? 1u : 0u);
+    for (int i = 0; i < 128; ++i) s[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t qa = smem_u32(sQ) + m * AT2_Q_BYTES + (ks >> 2) * (AT2_Q_BYTES / 2) + wg * 64 * 128;
+      const uint32_t ka = smem_u32(sK) + (ks >> 2) * (AT2_KV_BYTES / 2);
+      Wgmma<256>::ss(s, make_kmajor_desc<128>(qa) + (uint64_t)((ks & 3) * 2), make_kmajor_desc<128>(ka) + (uint64_t)((ks & 3) * 2), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // ---- softmax over the fragment: s[4i + 2h + j] = (row r0 + 8h, key 8i + c0 + j) ----
+    float nshift[2] = {kFolded ? 0.f : -P.shift_log2, kFolded ? 0.f : -P.shift_log2};
+    if constexpr (kExact) {
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          if (s_valid[8 * i + c0 + j]) {
+            mx[0] = fmaxf(mx[0], s[4 * i + j]);
+            mx[1] = fmaxf(mx[1], s[4 * i + 2 + j]);
           }
-          umma_commit(bar_s + m);
-        }
-        // ---- O_m = P_m V: A = P (bf16) from TMEM — keys 0..127 in cols [0,64), keys 128..255 in cols [192,256) —
-        //      B = V as MN-major smem operand, D = cols [64,192) ----
-        mbar_wait(bar_v, ph);
-        at2_stamp(P.trace, j, 0, 4);                 // V landed
-        for (int m = 0; m < n_mt; ++m) {
-          mbar_wait(bar_p + m, ph);
-          at2_stamp(P.trace, j, 0, 5 + m);           // P ready: PV issued
-          tc_fence_after();
-          const uint32_t R = tmem + m * 256;
 #pragma unroll
-          for (int ks = 0; ks < 16; ++ks) {          // 16 keys per instruction
-            const uint64_t vb = make_mnmajor_desc(smem_u32(sV) + ks * 16 * 128, (uint32_t)(AT2_KV_BYTES / 2), 1024u);
-            umma_f16_ts(R + 64, R + (ks < 8 ? ks * 8 : 192 + (ks - 8) * 8), vb, idesc_o, ks ? 1u : 0u);
-          }
-          umma_commit(bar_o + m);
-        }
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        nshift[h] = (mx[h] == -INFINITY) ? 0.f : -mx[h] * scale;
       }
     }
-  } else if (warp == 1) {
-    // ===================== TMA loader: Q/K of the next item as soon as both QK^T retired, V after both PV =====================
-    if (lane == 0) {
-      int j = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++j) {
-        const uint32_t prev = (j & 1) ^ 1;
-        const int head = w % P.heads, item = P.reverse ? P.items - 1 - w / P.heads : w / P.heads;
-        const int qc = P.q_col0 + head * 128, kc = P.k_col0 + head * 128, vc = P.v_col0 + head * 128;
-        if (j > 0)
-          for (int m = 0; m < n_mt; ++m) mbar_wait(bar_s + m, prev);
-        at2_stamp(P.trace, j, 1, 0);                 // Q/K buffers free: load issued
-        mbar_expect_tx(bar_qk0, AT2_Q_BYTES + AT2_KV_BYTES);
-        tma_load_3d(sQ, &tm_q, bar_qk0, qc, 0, item);
-        tma_load_3d(sQ + AT2_Q_BYTES / 2, &tm_q, bar_qk0, qc + 64, 0, item);
-        tma_load_3d(sK, &tm_k, bar_qk0, kc, 0, item);
-        tma_load_3d(sK + AT2_KV_BYTES / 2, &tm_k, bar_qk0, kc + 64, 0, item);
-        if (n_mt > 1) {
-          mbar_expect_tx(bar_q1, AT2_Q_BYTES);
-          tma_load_3d(sQ + AT2_Q_BYTES, &tm_q, bar_q1, qc, 128, item);
-          tma_load_3d(sQ + AT2_Q_BYTES + AT2_Q_BYTES / 2, &tm_q, bar_q1, qc + 64, 128, item);
-        }
-        if (j > 0)
-          for (int m = 0; m < n_mt; ++m) mbar_wait(bar_o + m, prev);
-        at2_stamp(P.trace, j, 1, 1);                 // V buffer free: load issued
-        mbar_expect_tx(bar_v, AT2_KV_BYTES);
-        tma_load_3d(sV, &tm_v, bar_v, vc, 0, item);
-        tma_load_3d(sV + AT2_KV_BYTES / 2, &tm_v, bar_v, vc + 64, 0, item);
+    float sum[2] = {0.f, 0.f};
+    uint32_t pk[64];   // P as bf16 pairs, already in the A-fragment order of the PV wgmma
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const bool v0 = s_valid[8 * i + c0] != 0, v1 = s_valid[8 * i + c0 + 1] != 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float x0 = kFolded ? s[4 * i + 2 * h] : fmaf(s[4 * i + 2 * h], scale, nshift[h]);
+        const float x1 = kFolded ? s[4 * i + 2 * h + 1] : fmaf(s[4 * i + 2 * h + 1], scale, nshift[h]);
+        float p0, p1;
+        if (((2 * i + h) & 7) < kPoly) { p0 = exp2_poly(x0); p1 = exp2_poly(x1); }
+        else { p0 = ex2_approx(x0); p1 = ex2_approx(x1); }
+        p0 = v0 ? p0 : 0.f;
+        p1 = v1 ? p1 : 0.f;
+        sum[h] += p0 + p1;
+        pk[2 * i + h] = pack_bf16(p0, p1);
       }
     }
-  } else if (warp == 2) {
-    // ===================== TMA storer: staging tile -> O[item, 128m.., head*128 ..] (rows >= T clipped) =====================
-    if (lane == 0) {
-      int j = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++j) {
-        const int head = w % P.heads, item = P.reverse ? P.items - 1 - w / P.heads : w / P.heads;
-        for (int m = 0; m < n_mt; ++m) {
-          mbar_wait(bar_full + m, j & 1);
-          at2_stamp(P.trace, j, 2, 2 * m);           // staging tile full
-          tma_store_3d(&tm_o, sO, head * 128, m * 128, item);
-          tma_store_3d(&tm_o, sO + AT2_O_BYTES / 2, head * 128 + 64, m * 128, item);
-          tma_store_commit();
-          tma_store_wait_read();          // the staging tile may be overwritten (by the other tile's epilogue)
-          at2_stamp(P.trace, j, 2, 2 * m + 1);       // staging tile read out
-          mbar_arrive(bar_free);
-        }
-      }
-      tma_store_wait_all();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
     }
-  } else if (((warp - 3) >> 3) < n_mt) {
-    // ===================== softmax / epilogue: thread = (query row, key half) =====================
-    const int m = (warp - 3) >> 3;                   // tile
-    const int q = warp & 3;                          // TMEM lane quarter this warp may access (warp id % 4)
-    const int h = ((warp - 3) >> 2) & 1;             // key half (softmax) = output-dim half (epilogue)
-    const int row = q * 32 + lane;
-    const uint32_t R = tmem + m * 256 + ((uint32_t)(q * 32) << 16);
-    const uint32_t S_h = R + 128 * h;                // this thread's 128 score columns
-    const uint32_t P_h = R + 192 * h;                // ... and where their 64 columns of packed P go
-    const uint32_t O_h = R + 64 + 64 * h;            // epilogue: output dims [64h, 64h + 64)
-    float* my_x = xch + (m * 2 + h) * 128 + row;
-    const float* peer_x = xch + (m * 2 + (h ^ 1)) * 128 + row;
-    const uint32_t stg = smem_u32(sO) + h * (AT2_O_BYTES / 2) + row * 128;
-    int j = 0;
-    for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++j) {
-      const uint32_t ph = j & 1;
-      const int item = P.reverse ? P.items - 1 - w / P.heads : w / P.heads;
-      // chunk order: ascending for the low key half, descending for the high half, so that each half's in-place P
-      // (16 columns per 32 keys) only ever overwrites score columns its own thread has already consumed
-      const int c0 = h ? 3 : 0, dc = h ? -1 : 1;
-      // validity bits of this thread's 128 keys (sequence end + padding mask), one ballot per 32 keys, in chunk order
-      uint32_t kbits[4];
-      {
-        const uint8_t* mk = P.key_mask ? P.key_mask + (long long)(P.mask_div > 1 ? item / P.mask_div : item) * P.T : nullptr;
+
+    // ---- O = P V: A fragment of key step ks = pk[4ks .. 4ks+3] (rows r0 / r0+8, keys 16ks + c0 / 16ks + 8 + c0) ----
+    mbar_wait(bar_v, 0);
+    float o[64];
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int key = h * 128 + (c0 + c * dc) * 32 + lane;
-          kbits[c] = __ballot_sync(0xffffffffu, key < P.T && (!mk || mk[key]));
-        }
-      }
-      mbar_wait(bar_s + m, ph);
-      if (lane == 0) at2_stamp(P.trace, j, warp, 0);   // S ready
-      tc_fence_after();
-      float nshift = -P.shift_log2;
-      if constexpr (kExact) {
-        // first pass: row maximum over this half, exchanged with the other half's thread of the same row
-        float mx = -INFINITY;
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          float v[32];
-          tmem_ld32(S_h + (c0 + c * dc) * 32, v);
-          tmem_ld_wait();
-          const uint32_t bits = kbits[c];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, (bits == 0xffffffffu || ((bits >> i) & 1u)) ? v[i] : -INFINITY);
-        }
-        *my_x = mx;
-        group_sync(m);
-        mx = fmaxf(mx, *peer_x);
-        group_sync(m);                  // both maxima are read before the slots are reused for the sums
-        nshift = (mx == -INFINITY) ? 0.f : -mx * P.scale_log2;
-      }
-      uint64_t sum2 = f2_pack(0.f, 0.f);
-      float va[32], vb[32];
-      uint32_t pk[16];
-      tmem_ld32(S_h + 32 * c0, va);
-      tmem_ld_wait();
-      tmem_ld32(S_h + 32 * (c0 + dc), vb);           // the next chunk's read runs under this chunk's arithmetic
-      softmax_chunk<kPoly, kFolded>(va, kbits[0], P.scale_log2, nshift, sum2, pk);
-      tmem_st16(P_h + 16 * c0, pk);
-      tmem_ld_wait();
-      tmem_ld32(S_h + 32 * (c0 + 2 * dc), va);
-      softmax_chunk<kPoly, kFolded>(vb, kbits[1], P.scale_log2, nshift, sum2, pk);
-      tmem_st16(P_h + 16 * (c0 + dc), pk);
-      tmem_ld_wait();
-      tmem_ld32(S_h + 32 * (c0 + 3 * dc), vb);
-      softmax_chunk<kPoly, kFolded>(va, kbits[2], P.scale_log2, nshift, sum2, pk);
-      tmem_st16(P_h + 16 * (c0 + 2 * dc), pk);
-      tmem_ld_wait();
-      softmax_chunk<kPoly, kFolded>(vb, kbits[3], P.scale_log2, nshift, sum2, pk);
-      tmem_st16(P_h + 16 * (c0 + 3 * dc), pk);
-      {
-        float s2a, s2b;
-        f2_unpack(sum2, s2a, s2b);
-        *my_x = s2a + s2b;
-      }
-      tmem_st_wait();
-      if (lane == 0) at2_stamp(P.trace, j, warp, 1);   // P written
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p + m);
-      // ---- epilogue: O[:, 64h .. 64h+64) / rowsum -> bf16 -> swizzled staging tile -> TMA store ----
-      mbar_wait(bar_o + m, ph);
-      if (lane == 0) at2_stamp(P.trace, j, warp, 2);   // O ready
-      tc_fence_after();
-      group_sync(m);                    // every thread of the group has published its half-row sum
-      if (lane == 0) at2_stamp(P.trace, j, warp, 3);
-      const float inv = 1.f / (*my_x + *peer_x);
-      tmem_ld32(O_h, va);
-      tmem_ld32(O_h + 32, vb);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_e + m);         // the tile's TMEM columns may be overwritten by the next QK^T
-      if (lane == 0) at2_stamp(P.trace, j, warp, 4);   // O in registers
-      const int use = j * n_mt + m;                  // staging-tile uses are ordered (item, tile)
-      if (use > 0) mbar_wait(bar_free, (use - 1) & 1);
-      if (lane == 0) at2_stamp(P.trace, j, warp, 5);   // staging tile free
-      const uint64_t inv2 = f2_pack(inv, inv);
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const float* s = (c < 4) ? &va[8 * c] : &vb[8 * (c - 4)];
-        uint32_t w4[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float a0, a1;
-          f2_unpack(f2_mul(f2_pack(s[2 * i], s[2 * i + 1]), inv2), a0, a1);
-          w4[i] = pack_bf16(a0, a1);
-        }
-        sts128u(stg + (uint32_t)((c ^ (row & 7)) << 4), make_uint4(w4[0], w4[1], w4[2], w4[3]));
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> TMA (async proxy) reads
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_full + m);
-      if (lane == 0) at2_stamp(P.trace, j, warp, 6);   // staged
+    for (int ks = 0; ks < 16; ++ks) {
+      const uint32_t a[4] = {pk[4 * ks], pk[4 * ks + 1], pk[4 * ks + 2], pk[4 * ks + 3]};
+      const uint64_t vb = make_mnmajor_desc(smem_u32(sV) + ks * 16 * 128, (uint32_t)(AT2_KV_BYTES / 2), 1024u);
+      wgmma_rs_n128_bmn(o, a, vb, 1u);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    reg_fence(pk);
+
+    // ---- epilogue: O / rowsum -> bf16 -> global (rows >= T dropped) ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m * 128 + wg * 64 + r0 + 8 * h;
+      if (row >= P.T) continue;
+      const float inv = 1.f / sum[h];
+      __nv_bfloat16* dst = P.o + ((long long)item * P.T + row) * P.o_ld + head * 128 + c0;
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+        *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+    }
   }
 }
 

@@ -1,5 +1,5 @@
 // SIMT kernels at the two 1-channel ends of the DAC-VAE codec, plus layout helpers.
-// The multi-channel convolutions run on the tcgen05 GEMM (gemm_tc.cuh) over channels-last audio.
+// The multi-channel convolutions run on the wgmma GEMM (gemm_tc.cuh) over channels-last audio.
 // (DAC-VAE arithmetic is restated from the Descript-DAC layout; reference call sites codec.py:65-89.)
 #pragma once
 #include "common.cuh"

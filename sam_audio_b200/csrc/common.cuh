@@ -1,5 +1,5 @@
-// sm_100a PTX wrappers shared by the SAM-Audio B200 kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), small math helpers.
+// sm_90a PTX wrappers shared by the SAM-Audio kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and shared-memory descriptors, small math helpers.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -58,77 +58,54 @@ SAB_DEVICE void tma_load_3d(void* smem, const CUtensorMap* m, uint64_t* bar, int
       : "memory");
 }
 
-// ----------------------------------------------------------------------------- tcgen05
-template <int kCols>
-SAB_DEVICE void tmem_alloc(uint32_t* smem_dst) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ----------------------------------------------------------------------------- wgmma
+// Order this thread's register / shared-memory writes before the warpgroup's next wgmma.mma_async.
+SAB_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+SAB_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+SAB_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// keep registers an asynchronous wgmma reads or writes where they are until the wgmma has retired
+template <int N>
+SAB_DEVICE void reg_fence(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-template <int kCols>
-SAB_DEVICE void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-SAB_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-SAB_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single issuing thread.
-SAB_DEVICE void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread retire
-// (implies tcgen05.fence::before_thread_sync).
-SAB_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <int N>
+SAB_DEVICE void reg_fence(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (base_lane + i).
-SAB_DEVICE void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-SAB_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// generic-proxy shared-memory writes -> reads by the async proxy (wgmma operands, TMA stores)
+SAB_DEVICE void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// barrier over a subset of the CTA's warps (ids 1..15; 0 is __syncthreads)
+SAB_DEVICE void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
-// Shared-memory matrix descriptor for a K-major bf16 tile whose rows are kRowBytes wide
-// (kRowBytes = 128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B) as written by a TMA box of that
-// inner extent; 8-row core-matrix groups are kRowBytes*8 apart (SBO).  Field layout follows
-// cute/arch/mma_sm100_desc.hpp (SmemDescriptor): start[0,14) lbo[16,30) sbo[32,46)
-// version[46,48)=1 layout_type[61,64).
+// Shared-memory matrix descriptor (sm_90 GMMA) for a K-major bf16 tile whose rows are kRowBytes wide
+// (kRowBytes = 128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B) as written by a TMA box of that inner extent;
+// 8-row core-matrix groups are kRowBytes*8 apart (SBO).  Fields: start[0,14) lbo[16,30) sbo[32,46)
+// layout_type[62,64) (1 = 128B, 2 = 64B, 3 = 32B swizzle).  Advancing 16 bf16 along K inside the swizzle row
+// adds 2 to the start field.
 template <int kRowBytes>
 SAB_DEVICE uint64_t make_kmajor_desc(uint32_t smem_addr) {
-  constexpr uint64_t layout = (kRowBytes == 128) ? 2ull : (kRowBytes == 64 ? 4ull : 6ull);
+  constexpr uint64_t layout = (kRowBytes == 128) ? 1ull : (kRowBytes == 64 ? 2ull : 3ull);
   constexpr uint64_t sbo = (uint64_t)(kRowBytes * 8) >> 4;
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;   // LBO: unused for swizzled K-major (one swizzle atom along K); canonical value 1
   d |= sbo << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-  d |= layout << 61;
+  d |= layout << 62;
   return d;
 }
-
-// Instruction descriptor, kind::f16: A=B=bf16, D=fp32, both K-major (mma_sm100_desc.hpp InstrDescriptor).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4)                    // c_format = F32
-         | (1u << 7)                  // a_format = BF16
-         | (1u << 10)                 // b_format = BF16
-         | ((uint32_t)(N >> 3) << 17) // n_dim
-         | ((uint32_t)(M >> 4) << 24);// m_dim
+// MN-major SWIZZLE_128B descriptor: 64-element (128 B) chunks along MN are `lbo` bytes apart, 8-row groups along K
+// are `sbo` bytes apart.
+SAB_DEVICE uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
 
 // explicit shared-window accesses (a pointer carved out of `extern __shared__` by byte arithmetic is a generic

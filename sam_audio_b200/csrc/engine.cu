@@ -14,7 +14,6 @@
 #include "../../include/samaudio_b200.h"
 #include "host_util.h"
 #include "attention.cuh"
-#include "attention_tc.cuh"
 #include "attention_tc2.cuh"
 #include "elementwise.cuh"
 #include "codec_kernels.cuh"
@@ -158,7 +157,7 @@ static GemmOp make_gemm(const char* tag, const AView& A, const bf16* B, int N, i
   memset(&op.P, 0, sizeof(op.P));
   op.tag = tag;
   op.BN = BN; op.BK = BK; op.mode = mode;
-  // 2-CTA pairs (cta_group::2, 256 x BN tiles) for the big tensor-bound GEMMs
+  // 2-CTA clusters (256 x BN tiles, B tile multicast to both CTAs) for the big tensor-bound GEMMs
   if (cg == 0) cg = (BN == 256 && BK == 64 && A.rows * A.items >= 1024 && A.rows >= 200) ? 2 : 1;
   if (g_force_cg && BN == 256 && BK == 64) cg = g_force_cg;
   op.cg = cg;
@@ -598,8 +597,7 @@ struct DitPlan {
   GemmOp g_y13, g_y2, g_in, g_xe[2], g_out, g_cond, g_mem, g_vid, g_kvc_all;
   std::vector<LayerOps> lay;
   CUtensorMap tm_att_q, tm_att_kv;   // fused-QKV buffer viewed as (3d cols, T rows, Bc items): box 64x128 / 64x256
-  CUtensorMap tm_att_o;              // attention output viewed as (d cols, T rows, Bc items): box 64x128 (TMA store)
-  bool att_tc = false;               // tcgen05 self-attention usable (T <= 256)
+  bool att_tc = false;               // wgmma self-attention usable (T <= 256)
   bool xa_fused = false;             // cross-attention folded into the cross.wq GEMM epilogue (L <= XA_MAX_TK)
   double flops_per_eval = 0;
   // the whole ODE solve (2*n_steps evaluations for midpoint, ~5.9k launches at 24 layers) as one CUDA graph, captured on the second solve
@@ -782,7 +780,6 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
   if (p.att_tc) {
     p.tm_att_q = make_tmap_3d(p.qkv, 3LL * d, T, Bc, 3LL * d, (int64_t)T * 3 * d, 64, 128);
     p.tm_att_kv = make_tmap_3d(p.qkv, 3LL * d, T, Bc, 3LL * d, (int64_t)T * 3 * d, 64, 256);
-    p.tm_att_o = make_tmap_3d(p.att, d, T, Bc, d, (int64_t)T * d, 64, 128);
   }
 
   // algorithmic FLOPs of one evaluation (GEMMs + attention), for roofline reporting
@@ -832,16 +829,6 @@ static void attention(sab_engine* e, const AttnParams& ap, int items, int heads,
   SAB_CUDA(cudaGetLastError());
 }
 
-static void launch_attention_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnTcParams& ap,
-                                int items, cudaStream_t st) {
-  ensure_dynamic_smem(reinterpret_cast<const void*>(attention_tc_kernel), ATC_SMEM);
-  AttnTcParams p2 = ap;
-  p2.items = items;
-  const int n_work = ap.heads * items;
-  attention_tc_kernel<<<n_work < sm_count() ? n_work : sm_count(), ATC_THREADS, ATC_SMEM, st>>>(tq, tk, tv, p2);
-  SAB_CUDA(cudaGetLastError());
-}
-
 // algorithmic HBM bytes of one GEMM launch: operands once + every epilogue stream once (what a perfect kernel moves)
 static double gemm_bytes(const GemmOp& op) {
   const GemmParams& P = op.P;
@@ -853,26 +840,25 @@ static double gemm_bytes(const GemmOp& op) {
   const double n_out = (op.mode == EPI_SWIGLU) ? P.N / 2.0 : (double)P.N;
   return op.in_bytes + op.rows * n_out * per_elem;
 }
-// second-generation tcgen05 self-attention (attention_tc2.cuh).  shift_log2 < 0 selects the exact two-pass softmax.
+// wgmma self-attention (attention_tc2.cuh).  shift_log2 < 0 selects the exact two-pass softmax.
 static int g_attn_poly = 2;      // SAB_ATTN_POLY=0..4: pairs of every 8 whose exponential runs on the FMA pipe
 template <bool kExact, int kPoly, bool kFolded>
 static void launch_attention_tc2_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
-                                      const CUtensorMap& to, const AttnTc2Params& ap, cudaStream_t st) {
+                                      const AttnTc2Params& ap, cudaStream_t st) {
   auto kern = attention_tc2_kernel<kExact, kPoly, kFolded>;
   ensure_dynamic_smem(reinterpret_cast<const void*>(kern), AT2_SMEM);
-  const int n_work = ap.heads * ap.items;
-  kern<<<n_work < sm_count() ? n_work : sm_count(), AT2_THREADS, AT2_SMEM, st>>>(tq, tk, tv, to, ap);
+  kern<<<ap.heads * ap.items, AT2_THREADS, AT2_SMEM, st>>>(tq, tk, tv, ap);
   SAB_CUDA(cudaGetLastError());
 }
 // variants: exact (two-pass row maximum; shift_log2 < 0), single pass with scale and shift, and `folded`
 // (scale already in q, |logit| <= 50: p = 2^s) — the engine's production path
-static void launch_attention_tc2(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& to,
+static void launch_attention_tc2(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                                  const AttnTc2Params& ap, bool folded, cudaStream_t st) {
   const bool exact = ap.shift_log2 < 0.f;
   SAB_CHECK(!(exact && folded), "folded softmax needs a logit bound");
-#define SAB_AT2(p_) case p_: return exact ? launch_attention_tc2_inst<true, p_, false>(tq, tk, tv, to, ap, st)   \
-                                  : folded ? launch_attention_tc2_inst<false, p_, true>(tq, tk, tv, to, ap, st)  \
-                                           : launch_attention_tc2_inst<false, p_, false>(tq, tk, tv, to, ap, st);
+#define SAB_AT2(p_) case p_: return exact ? launch_attention_tc2_inst<true, p_, false>(tq, tk, tv, ap, st)   \
+                                  : folded ? launch_attention_tc2_inst<false, p_, true>(tq, tk, tv, ap, st)  \
+                                           : launch_attention_tc2_inst<false, p_, false>(tq, tk, tv, ap, st);
   switch (g_attn_poly) {
     SAB_AT2(0) SAB_AT2(2) SAB_AT2(3) SAB_AT2(4)
     default: throw Error(fmt("SAB_ATTN_POLY=%d not built (0, 2, 3, 4)", g_attn_poly));
@@ -884,7 +870,7 @@ static void gemm(sab_engine* e, const GemmOp& op, cudaStream_t st) {
   mark(e, st, op.tag, op.flops, gemm_bytes(op));
   launch_gemm(op, st);
 }
-// Serpentine row order.  Every kernel of a DiT layer is row-parallel and streams activations that exceed the 126 MB
+// Serpentine row order.  Every kernel of a DiT layer is row-parallel and streams activations that exceed the 50 MB
 // L2 (fp32 residual 180 MB, fused QKV 270 MB, FFN hidden 241 MB at B = 64): a consumer that walks the rows in the
 // same direction as its producer finds the first rows evicted.  Alternating the direction from one launch to the
 // next makes each kernel start on the rows its producer wrote last, so roughly an L2's worth of its input (and of the
@@ -988,9 +974,9 @@ static void dit_eval(sab_engine* e, const float* time_dev, const FinalSpec& fs, 
     a.v = p.qkv; a.v_ld = 3 * d; a.v_col0 = 2 * d;
     a.o = p.att; a.o_ld = d; a.key_mask = p.pad_mask; a.Tq = T; a.Tk = T; a.mask_div = cand;
     a.scale_log2 = 1.f;          // self-attention: log2(e)/sqrt(hd) is folded into q by the QKV epilogue (W.qn_scaled)
-    static const bool attn_v1 = getenv("SAB_ATTN_V1") != nullptr;   // A/B against the first-generation kernel
-    if (p.att_tc && !attn_v1) {
+    if (p.att_tc) {
       AttnTc2Params tp{};
+      tp.o = p.att; tp.o_ld = d;
       tp.key_mask = p.pad_mask; tp.T = T; tp.heads = H; tp.items = Bc; tp.mask_div = cand;
       // the softmax scale is already in q (QKV epilogue, W.qn_scaled): scale 1 for the exact fallback, and with a
       // logit bound the folded single-pass kernel needs neither scale nor shift
@@ -998,13 +984,7 @@ static void dit_eval(sab_engine* e, const float* time_dev, const FinalSpec& fs, 
       tp.reverse = g_serpentine ? dir : 0;
       dir ^= 1;
       mark(e, st, "sdpa.self", 4.0 * Bc * H * (double)T * T * 128, (double)M * 4.0 * d * 2.0);   // reads q|k|v, writes o (bf16)
-      launch_attention_tc2(p.tm_att_q, p.tm_att_kv, p.tm_att_kv, p.tm_att_o, tp, W.att_shift_log2 >= 0.f, st);
-    } else if (p.att_tc) {
-      AttnTcParams tp{};
-      tp.o = p.att; tp.o_ld = d; tp.key_mask = p.pad_mask; tp.Tq = T; tp.Tk = T; tp.heads = H; tp.mask_div = cand;
-      tp.q_col0 = 0; tp.k_col0 = d; tp.v_col0 = 2 * d; tp.scale_log2 = 1.f; tp.v_lbo = ATC_KV_BYTES / 2; tp.v_sbo = 1024;
-      mark(e, st, "sdpa.self", 4.0 * Bc * H * (double)T * T * 128, 0);
-      launch_attention_tc(p.tm_att_q, p.tm_att_kv, p.tm_att_kv, tp, Bc, st);
+      launch_attention_tc2(p.tm_att_q, p.tm_att_kv, p.tm_att_kv, tp, W.att_shift_log2 >= 0.f, st);
     } else {
       attention(e, a, Bc, H, st);
     }
@@ -1313,13 +1293,14 @@ int sab_create(const sab_config* cfg, int device, sab_engine** out) {
   SAB_CHECK(cfg && out, "null argument");
   int n_dev = 0;
   cudaError_t ce = cudaGetDeviceCount(&n_dev);
-  SAB_CHECK(ce == cudaSuccess && n_dev > 0, "no CUDA device: the SAM-Audio B200 path has no CPU fallback (%s)",
+  SAB_CHECK(ce == cudaSuccess && n_dev > 0, "no CUDA device: the SAM-Audio GPU path has no CPU fallback (%s)",
             cudaGetErrorString(ce));
   SAB_CHECK(device >= 0 && device < n_dev && device < kMaxDevices, "bad device index %d", device);
   DeviceGuard _dg(device);
   cudaDeviceProp prop;
   SAB_CUDA(cudaGetDeviceProperties(&prop, device));
-  SAB_CHECK(prop.major == 10, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  SAB_CHECK(prop.major == 9 && prop.minor == 0, "device %d is sm_%d%d; this library is built for sm_90a only", device,
+            prop.major, prop.minor);
   if (const char* f = getenv("SAB_FORCE_CG")) g_force_cg = atoi(f);
   if (const char* f = getenv("SAB_ATTN_POLY")) g_attn_poly = atoi(f);
   g_serpentine = getenv("SAB_NO_SERPENTINE") == nullptr;
@@ -1830,45 +1811,26 @@ int sab_test_attention(int items, int heads, int Tq, int Tk, const void* q, cons
   SAB_API_END
 }
 
-int sab_test_attention_tc(int items, int heads, int T, const void* q, const void* k, const void* v,
-                          const uint8_t* key_mask, void* o, int v_lbo, int v_sbo, void* stream) {
-  SAB_API_BEGIN
-  SAB_CHECK(T <= 256, "tcgen05 attention handles T <= 256");
-  const long long ld = (long long)heads * 128;
-  CUtensorMap tq = make_tmap_3d(q, ld, T, items, ld, (int64_t)T * ld, 64, 128);
-  CUtensorMap tk = make_tmap_3d(k, ld, T, items, ld, (int64_t)T * ld, 64, 256);
-  CUtensorMap tv = make_tmap_3d(v, ld, T, items, ld, (int64_t)T * ld, 64, 256);
-  AttnTcParams tp{};
-  tp.o = (bf16*)o; tp.o_ld = ld; tp.key_mask = key_mask; tp.Tq = T; tp.Tk = T; tp.heads = heads;
-  tp.q_col0 = tp.k_col0 = tp.v_col0 = 0;
-  tp.scale_log2 = (1.0f / sqrtf(128.f)) * 1.4426950408889634f;
-  tp.v_lbo = v_lbo > 0 ? v_lbo : ATC_KV_BYTES / 2;
-  tp.v_sbo = v_sbo > 0 ? v_sbo : 1024;
-  launch_attention_tc(tq, tk, tv, tp, items, (cudaStream_t)stream);
-  SAB_API_END
-}
-
 int sab_test_attention_tc2(int items, int heads, int T, const void* q, const void* k, const void* v,
-                           const uint8_t* key_mask, void* o, float shift_log2, int poly, long long* trace, void* stream) {
+                           const uint8_t* key_mask, void* o, float shift_log2, int poly, void* stream) {
   SAB_API_BEGIN
-  SAB_CHECK(T <= 256 && T >= 1, "tcgen05 attention handles 1 <= T <= 256");
+  SAB_CHECK(T <= 256 && T >= 1, "wgmma attention handles 1 <= T <= 256");
   const long long ld = (long long)heads * 128;
   CUtensorMap tq = make_tmap_3d(q, ld, T, items, ld, (int64_t)T * ld, 64, 128);
   CUtensorMap tk = make_tmap_3d(k, ld, T, items, ld, (int64_t)T * ld, 64, 256);
   CUtensorMap tv = make_tmap_3d(v, ld, T, items, ld, (int64_t)T * ld, 64, 256);
-  CUtensorMap to = make_tmap_3d(o, ld, T, items, ld, (int64_t)T * ld, 64, 128);
   AttnTc2Params tp{};
+  tp.o = (bf16*)o; tp.o_ld = ld;
   tp.key_mask = key_mask; tp.T = T; tp.heads = heads; tp.items = items; tp.mask_div = 1;
   tp.q_col0 = tp.k_col0 = tp.v_col0 = 0;
   tp.scale_log2 = (1.0f / sqrtf(128.f)) * 1.4426950408889634f;
   tp.shift_log2 = shift_log2;
-  tp.trace = trace;
   const int saved = g_attn_poly;
   if (poly >= 0) g_attn_poly = poly;
   try {
     // shift_log2 == 0: folded path (the caller passes q already multiplied by log2(e)/sqrt(hd), |logit| <= 50)
     if (shift_log2 == 0.f) tp.shift_log2 = 50.f;
-    launch_attention_tc2(tq, tk, tv, to, tp, shift_log2 == 0.f, (cudaStream_t)stream);
+    launch_attention_tc2(tq, tk, tv, tp, shift_log2 == 0.f, (cudaStream_t)stream);
   } catch (...) {
     g_attn_poly = saved;
     throw;

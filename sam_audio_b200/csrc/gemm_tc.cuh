@@ -1,23 +1,23 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:   D[m, n] = sum_k A[m', k'] * B[n, k]
+// Persistent, warp-specialised wgmma GEMM for sm_90a:   D[m, n] = sum_k A[m', k'] * B[n, k]
 //
 //  * A (activations, bf16, K-major rows) arrives through a 3-D TMA map (cols, rows-per-item, items);
 //    the K loop is a short list of "runs" (row_shift, a_col, n k-blocks), so the same kernel serves
 //    plain linears (1 run), dilated / strided Conv1d and ConvTranspose1d over channels-last audio
 //    (one run per tap; TMA zero-fills rows that fall off either end of an item = the conv's padding).
 //  * B (weights, bf16, [N, Ktot] K-major, packed at load time) arrives through a 2-D TMA map.
-//  * Accumulators live in TMEM (2 x BN fp32 columns, double buffered): the epilogue of tile i
-//    overlaps the MMAs of tile i+1.  One elected thread issues tcgen05.mma (K=16 per instruction).
-//  * CG = 1: one CTA per 128 x BN tile (M=128 UMMA).
-//    CG = 2: a 2-CTA cluster (one TPC) per 256 x BN tile: tcgen05.mma.cta_group::2 (M=256) issued by the
-//    leader CTA; each CTA stages its own 128 A rows and HALF of the B tile, so B's L2->SMEM traffic and
-//    shared-memory fill per SM halve.  TMA of both CTAs signals the leader's "full" barrier; tcgen05.commit
-//    multicasts "slot free" / "accumulator ready" to both CTAs; epilogue warps of both CTAs release the
-//    accumulator on the leader's barrier.
-//  * Warp roles: 0 = TMA producer, 1 = MMA issuer, 2 = TMEM allocator, 4..11 = epilogue, two warps per
-//    TMEM lane quarter taking alternating 32-column chunks
-//    (warp w reads TMEM lanes 32*(w%4).. : thread <-> output row), then transposes 32x32 fp32 blocks
-//    through a padded shared-memory staging tile so that every global access is row-contiguous
-//    (8 lanes x 16 B = one full 128 B line per row).
+//  * Warp 0 is the TMA producer (a ring of mbarrier-guarded stages); warps 4..11 form two consumer
+//    warpgroups.  Warpgroup g multiplies rows 64g .. 64g+63 of the 128 x BN tile with wgmma.mma_async
+//    (m64nBNk16, both operands from shared memory, fp32 accumulators in registers, one k-block in flight),
+//    then writes its accumulators into an fp32 [128 x BN] shared-memory tile (16-byte units XOR-swizzled
+//    by row, conflict-free for both access patterns below).  The same eight warps run the epilogue from
+//    that tile, two warps per 32-row quarter taking alternating 32-column chunks: a thread reads one row's
+//    32 values, or a transposed 4-column x 8-row block so that every global access is row-contiguous
+//    (8 lanes x 16 B = one full 128 B line per row).  The producer refills the stages with the next tile
+//    while the epilogue runs.
+//  * CG = 1: one CTA per 128 x BN tile.
+//    CG = 2: a 2-CTA cluster per 256 x BN tile: each CTA stages its own 128 A rows and loads HALF of the B
+//    tile, multicast into both CTAs' shared memory, so B's L2 -> SMEM traffic per SM halves.  A stage is
+//    refilled only when the consumers of both CTAs have released it (remote mbarrier arrives).
 //  * Tiles are rasterised in groups of `group_m` m-tiles that sweep n: the A panel of a group stays in L2.
 //  * Epilogues (fused, no extra pass over HBM):
 //      EPI_AFFINE : v = (acc + bias[n]) * gate[row/gate_div, n] * alpha + res[row, n]
@@ -26,11 +26,12 @@
 //      EPI_QKV    : per-head RMSNorm (q,k) + RoPE on adjacent pairs -> bf16   (heads are 128 contiguous cols)
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace sab {
 
 constexpr int GEMM_BM = 128;
-constexpr int GEMM_THREADS = 384;   // 4 role warps + 8 epilogue warps
+constexpr int GEMM_THREADS = 384;   // warp 0: TMA producer, warps 1..3 idle, warps 4..11: two consumer warpgroups
 constexpr int GEMM_MAX_RUNS = 8;
 
 // EPI_AFFINE_NORM = EPI_AFFINE + the producer half of the fused RMSNorm (own instantiation: the extra per-lane state
@@ -97,18 +98,17 @@ constexpr int XA_MAX_TK = 8;
 template <int BN, int BK, int CG, bool B2B = false>
 struct GemmSmem {
   static constexpr int kABytes = GEMM_BM * BK * 2;
-  static constexpr int kBBytes = (BN / CG) * BK * 2;
+  static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStageLd = 36;                          // fp32 words per staged row (32 + 4 pad)
-  static constexpr int kEpiBytes = 8 * 32 * kStageLd * 4;      // 8 epilogue warps x 32 rows
+  static constexpr int kAccBytes = GEMM_BM * BN * 4;          // fp32 accumulator tile handed to the epilogue
   static constexpr int kBarBytes = 1024;
   // back-to-back second GEMM (1x1 conv of a residual unit): its [BN x BN] weight stays resident and the activated
   // 128 x BN intermediate tile is handed to the tensor core through shared memory, both K-major swizzled
   static constexpr int kW1Bytes = B2B ? BN * BN * 2 : 0;
   static constexpr int kMidBytes = B2B ? GEMM_BM * BN * 2 : 0;
-  static constexpr int kBudget = 227 * 1024 - kEpiBytes - kBarBytes - 1024 - kW1Bytes - kMidBytes;
+  static constexpr int kBudget = 227 * 1024 - kAccBytes - kBarBytes - 1024 - kW1Bytes - kMidBytes;
   static constexpr int kStages = kBudget / kStageBytes > 8 ? 8 : kBudget / kStageBytes;
-  static constexpr int kTotal = kStages * kStageBytes + kW1Bytes + kMidBytes + kBarBytes + kEpiBytes + 1024;  // +1024: alignment
+  static constexpr int kTotal = kStages * kStageBytes + kW1Bytes + kMidBytes + kAccBytes + kBarBytes + 1024;  // +1024: alignment
 };
 
 // ---- cluster helpers (CG = 2) ----
@@ -125,48 +125,18 @@ SAB_DEVICE void cluster_sync_all() {
 SAB_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  // default semantics (release at CTA scope): the accumulator hand-over is ordered by tcgen05.fence::before_thread_sync;
-  // a cluster-scope release would make every epilogue warp wait for its outstanding global stores (MEMBAR.GPU + ERRBAR)
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit: address of the leader CTA's barrier
-SAB_DEVICE void tma_load_2d_cg2(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
+// TMA load written to the same offset in every CTA of `mask`; each destination CTA's mbarrier at `bar`'s offset
+// receives the bytes it got
+SAB_DEVICE void tma_load_2d_mc(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-SAB_DEVICE void tma_load_3d_cg2(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1),
-      "r"(c2)
-      : "memory");
-}
-SAB_DEVICE void umma_f16_cg2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-SAB_DEVICE void umma_commit_cg2(uint64_t* bar) {  // arrive on `bar` in both CTAs of the pair
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-template <int kCols>
-SAB_DEVICE void tmem_alloc_cg2(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-SAB_DEVICE void tmem_dealloc_cg2(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+SAB_DEVICE void sts64(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 
 // tile -> (unit m-tile, n-tile): groups of `group_m` m-tiles sweep n (m fastest inside a group)
@@ -191,34 +161,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   using S = GemmSmem<BN, BK, CG, B2B>;
   static_assert(!B2B || (CG == 1 && MODE == EPI_AFFINE && BN <= 128), "back-to-back mode: 1-CTA affine tiles, N <= 128");
   constexpr int kStages = S::kStages;
-  constexpr int kLd = S::kStageLd;
-  constexpr int kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  constexpr int kAccStride = (BN <= 64) ? 64 : (BN <= 128) ? 128 : 256;  // column offset of accumulator 1
-  static_assert(2 * kAccStride <= 512, "accumulators exceed TMEM");
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "invalid UMMA N");
+  static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "invalid wgmma N / epilogue chunking");
   static_assert(BK == 64 || BK == 32, "BK must be one swizzle row (128B or 64B)");
-  static_assert(CG == 1 || CG == 2, "cta group");
+  static_assert(CG == 1 || (CG == 2 && BN % 16 == 0), "cta group");
   static_assert(kStages >= 2, "pipeline too shallow");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_w1 = smem + kStages * S::kStageBytes;            // [BN/BK chunks][BN rows x BK] (B2B)
   uint8_t* s_mid = s_w1 + S::kW1Bytes;                         // [BN/BK chunks][128 rows x BK] (B2B)
-  uint8_t* bar_base = s_mid + S::kMidBytes;
+  uint8_t* s_acc = s_mid + S::kMidBytes;                       // fp32 [128 x BN], swizzled
+  uint8_t* bar_base = s_acc + S::kAccBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bar_base);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* b2b_full = tmem_empty + 2;      // [2] second GEMM retired into accumulator a
-  uint64_t* mid_ready = b2b_full + 2;       // all epilogue warps have written the intermediate tile
-  uint64_t* w1_bar = mid_ready + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w1_bar + 1);
-  float* epi_stage = reinterpret_cast<float*>(bar_base + S::kBarBytes);
+  uint64_t* w1_bar = empty_bar + kStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const uint32_t cta_rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const bool leader = cta_rank == 0;
   const int unit = blockIdx.x / CG, n_units = gridDim.x / CG;
   const int n_tiles_m = P.n_items * P.tiles_per_item;
   const int n_tiles = n_tiles_m * P.n_tiles_n;
@@ -226,33 +186,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8 * CG);   // one arrive per consumer warp of every CTA that reads the stage's B
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 8 * CG);  // one arrive per epilogue warp of every CTA of the group
-      mbar_init(&b2b_full[a], 1);
-    }
-    mbar_init(mid_ready, 8);
     mbar_init(w1_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (CG == 2) tmem_alloc_cg2<kTmemCols>(tmem_slot);
-    else tmem_alloc<kTmemCols>(tmem_slot);
-  }
-  tc_fence_before();
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(smem_u32(tmem_slot)));
-  // consume the loaded value here: otherwise its first use sits inside the epilogue's chunk loop and every iteration
-  // waits on the load's scoreboard slot, which by then tracks the residual prefetches (ncu: 18% of the epilogue's time)
-  if (tmem_base == 0xFFFFFFFFu) __trap();
 
   if (warp == 0) {
     // ===================== TMA producer (every CTA) =====================
@@ -278,98 +219,69 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* sa = smem + stage * S::kStageBytes;
             uint8_t* sb = sa + S::kABytes;
-            if constexpr (CG == 2) {
-              if (leader) mbar_expect_tx(&full_bar[stage], 2 * S::kStageBytes);
-              tma_load_3d_cg2(sa, &tmA, &full_bar[stage], run.a_col + kb * BK, t0 + run.row_shift, item);
-              tma_load_2d_cg2(sb, &tmB, &full_bar[stage], kb_global * BK, nb);
-            } else {
-              mbar_expect_tx(&full_bar[stage], S::kStageBytes);
-              tma_load_3d(sa, &tmA, &full_bar[stage], run.a_col + kb * BK, t0 + run.row_shift, item);
+            mbar_expect_tx(&full_bar[stage], S::kStageBytes);
+            tma_load_3d(sa, &tmA, &full_bar[stage], run.a_col + kb * BK, t0 + run.row_shift, item);
+            if constexpr (CG == 2)
+              tma_load_2d_mc(sb + cta_rank * (BN / 2) * BK * 2, &tmB, &full_bar[stage], kb_global * BK, nb, (uint16_t)3);
+            else
               tma_load_2d(sb, &tmB, &full_bar[stage], kb_global * BK, nb);
-            }
             if (++stage == kStages) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = make_idesc_bf16(GEMM_BM * CG, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      // back-to-back: the second GEMM of tile i is issued as soon as the epilogue warps have published the
-      // activated intermediate tile — polled between the k-blocks of tile i+1, at the latest before tile i+1 commits
-      int pend_acc = -1;
-      uint32_t mid_phase = 0;
-      bool w1_loaded = false;
-      auto issue_b2b = [&](int a) {
-        if (!w1_loaded) { mbar_wait(w1_bar, 0); w1_loaded = true; }
-        tc_fence_after();
-        const uint32_t d2 = tmem_base + a * kAccStride;
-#pragma unroll
-        for (int kc = 0; kc < BN / BK; ++kc) {
-          const uint64_t dm = make_kmajor_desc<BK * 2>(smem_u32(s_mid + kc * (GEMM_BM * BK * 2)));
-          const uint64_t dw = make_kmajor_desc<BK * 2>(smem_u32(s_w1 + kc * (BN * BK * 2)));
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) umma_f16(d2, dm + (uint64_t)(k * 2), dw + (uint64_t)(k * 2), idesc, (kc | k) ? 1u : 0u);
-        }
-        umma_commit(&b2b_full[a]);
-      };
-      for (int tile = unit; tile < n_tiles; tile += n_units) {
-        int mt, nt;
-        tile_coords(tile, n_tiles_m, P.n_tiles_n, P.group_m, P.reverse_m, mt, nt);
-        const int n0 = nt * BN;
-        const int list = (P.n_period > 0 && (n0 % P.n_period) >= P.n_switch) ? 1 : 0;
-        int total_kb = 0;
-        for (int r = 0; r < P.n_runs[list]; ++r) total_kb += P.runs[list][r].nkb;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccStride;
-        for (int kb = 0; kb < total_kb; ++kb) {
-          if constexpr (B2B) {
-            if (pend_acc >= 0 && mbar_try_wait(mid_ready, mid_phase)) { issue_b2b(pend_acc); pend_acc = -1; mid_phase ^= 1; }
-          }
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
-          const uint32_t sb = sa + S::kABytes;
-          const uint64_t da = make_kmajor_desc<BK * 2>(sa);
-          const uint64_t db = make_kmajor_desc<BK * 2>(sb);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 bf16 = 32 B along K inside the swizzle row: +2 in the (addr >> 4) field
-            if constexpr (CG == 2) umma_f16_cg2(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-            else umma_f16(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-          }
-          if constexpr (CG == 2) umma_commit_cg2(&empty_bar[stage]); else umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        if constexpr (B2B) {
-          if (pend_acc >= 0) { mbar_wait(mid_ready, mid_phase); issue_b2b(pend_acc); pend_acc = -1; mid_phase ^= 1; }
-        }
-        if constexpr (CG == 2) umma_commit_cg2(&tmem_full[acc]); else umma_commit(&tmem_full[acc]);
-        if constexpr (B2B) pend_acc = acc;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if constexpr (B2B) {
-        if (pend_acc >= 0) { mbar_wait(mid_ready, mid_phase); issue_b2b(pend_acc); }
-      }
-    }
   } else if (warp >= 4) {
-    // ===================== epilogue (every CTA): 8 warps, 2 per TMEM lane quarter =====================
-    // Two warps share each SM sub-partition so one can issue while the other waits on TMEM / shared / global
-    // latency; every inner loop is straight-line (8 independent rows per lane) so the compiler can overlap them.
+    // ===================== consumers: wgmma main loop, then the epilogue (8 warps, 2 per 32-row quarter) =====================
     const int e = warp - 4;                    // 0..7
-    const int q = e & 3;                       // TMEM lane quarter (== warp % 4)
+    const int q = e & 3;                       // 32-row quarter of the tile this warp's epilogue covers
     const int half = e >> 2;                   // which alternating 32-column chunks this warp owns
-    const uint32_t stg = smem_u32(epi_stage) + (uint32_t)(e * 32 * kLd * 4);   // this warp's staging tile (shared window)
+    const int wg = e >> 2;                     // consumer warpgroup: wgmma rows 64 wg .. 64 wg + 63
     const int tr_r = lane >> 3;                // transposed mapping: pass p covers row 4p + tr_r,
     const int tr_c = (lane & 7) * 4;           //   4 consecutive columns tr_c .. tr_c+3
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    const uint32_t acc_base = smem_u32(s_acc);
+    const int arow = q * 32 + lane;            // this thread's row in the row-per-thread epilogue form
+    // byte address of (row, col) in the accumulator tile: 16-byte unit (col / 4) XOR (row % 8)
+    auto acc_addr = [&](int r, int col) -> uint32_t {
+      return acc_base + (uint32_t)(r * BN * 4) + (uint32_t)((((col >> 2) ^ (r & 7))) << 4) + (uint32_t)((col & 3) * 4);
+    };
+    // 32 consecutive columns c .. c+31 of this thread's row
+    auto acc_ld32 = [&](int c, float (&v)[32]) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 t = lds128(acc_addr(arow, c + 4 * j));
+        v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
+      }
+    };
+    // overwrite them (values derived from this thread's own row, read back transposed below)
+    auto acc_put = [&](int c, const float (&v)[32]) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sts128(acc_addr(arow, c + 4 * j), make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+      __syncwarp();
+    };
+    // transposed read of the warp's 32 x 32 block at column c: pass p = row q*32 + 4p + tr_r, columns c + tr_c .. +3
+    auto acc_get = [&](int c, float4 (&x)[8]) {
+#pragma unroll
+      for (int p = 0; p < 8; ++p) x[p] = lds128(acc_addr(q * 32 + 4 * p + tr_r, c + tr_c));
+    };
+    float accr[BN / 2];
+    // this warpgroup's accumulator fragment -> the shared tile (rows 64 wg + 16 (warp % 4) + lane / 4 [+ 8])
+    auto acc_dump = [&]() {
+      const int r0 = wg * 64 + (e & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = 8 * i + 2 * (lane & 3);
+        sts64(acc_addr(r0, col), accr[4 * i], accr[4 * i + 1]);
+        sts64(acc_addr(r0 + 8, col), accr[4 * i + 2], accr[4 * i + 3]);
+      }
+    };
+    auto release = [&](int s) {
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if constexpr (CG == 2) mbar_arrive_cluster(&empty_bar[s], cta_rank ^ 1u);
+      }
+    };
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = unit; tile < n_tiles; tile += n_units) {
       int mt, nt;
       tile_coords(tile, n_tiles_m, P.n_tiles_n, P.group_m, P.reverse_m, mt, nt);
@@ -378,7 +290,36 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const long long row0 = (long long)item * P.rows_per_item + t_base + tr_r;   // this lane's row in pass 0
       const int rl = P.rows_per_item - t_base - tr_r;   // pass p is valid iff 4p < rl
       const int n0 = nt * BN;
-      const uint32_t t_addr = tmem_base + acc * kAccStride + ((uint32_t)(q * 32) << 16);
+
+      // ---- main loop: one k-block of wgmma in flight; a stage is released once the wgmma reading it retired ----
+      {
+        const int list = (P.n_period > 0 && (n0 % P.n_period) >= P.n_switch) ? 1 : 0;
+        int total_kb = 0;
+        for (int r = 0; r < P.n_runs[list]; ++r) total_kb += P.runs[list][r].nkb;
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) accr[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < total_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
+          const uint64_t da = make_kmajor_desc<BK * 2>(sa + (uint32_t)(wg * 64 * BK * 2));
+          const uint64_t db = make_kmajor_desc<BK * 2>(sa + S::kABytes);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) Wgmma<BN>::ss(accr, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          reg_fence(accr);
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        reg_fence(accr);
+        if (prev >= 0) release(prev);
+      }
+      acc_dump();
+      named_bar_sync(1, 256);
 
       // fused-RMSNorm consumer: rstd and the per-item bias row of THIS LANE'S row (thread == row form); the loads are
       // issued before the accumulator wait
@@ -393,18 +334,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         nrm_rstd = rsqrtf(ssum * P.ssq_inv_dim + P.eps);
         nrm_brow = P.ibias + (long long)((uint32_t)grow / (uint32_t)P.ibias_div) * P.ibias_ld + n0;
       }
-
-      // write this thread's 32 accumulator values (one row) into the staging tile, then read them back transposed
-      auto stage_put = [&](const float (&v)[32]) {
-        const uint32_t dst = stg + (uint32_t)(lane * kLd * 4);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sts128(dst + 16 * j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
-        __syncwarp();
-      };
-      auto stage_get = [&](float4 (&x)[8]) {
-#pragma unroll
-        for (int p = 0; p < 8; ++p) x[p] = lds128(stg + (uint32_t)(((4 * p + tr_r) * kLd + tr_c) * 4));
-      };
 
       constexpr bool kNorm = (MODE == EPI_AFFINE_NORM);
       if constexpr (MODE == EPI_AFFINE || MODE == EPI_AFFINE_NORM) {
@@ -435,14 +364,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         if constexpr (B2B) {
           // ---- first epilogue: Snake(acc0 + bias) -> bf16 -> the K-major swizzled A tile of the second GEMM ----
-          mbar_wait(&tmem_full[acc], acc_phase);
-          tc_fence_after();
           const int r_tile = q * 32 + lane;                    // row of this thread inside the 128-row tile
 #pragma unroll 1
           for (int c = half * 32; c < BN; c += 64) {
             float v[32];
-            tmem_ld32(t_addr + c, v);
-            tmem_ld_wait();
+            acc_ld32(c, v);
             uint32_t pk[16];
 #pragma unroll
             for (int j = 0; j < 32; j += 4) {
@@ -456,7 +382,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               pk[j >> 1] = pack_bf16(x0, x1);
               pk[(j >> 1) + 1] = pack_bf16(x2, x3);
             }
-            // chunk of BK columns kc, 16-byte unit u inside the row, XOR-swizzled like the TMA/UMMA layout
+            // chunk of BK columns kc, 16-byte unit u inside the row, XOR-swizzled like the TMA layout
             const uint32_t tile = smem_u32(s_mid) + (uint32_t)((c / BK) * (GEMM_BM * BK * 2) + r_tile * (BK * 2));
             const int u0 = (c % BK) / 8;
             const int sw = (BK == 64) ? (r_tile & 7) : ((r_tile >> 1) & 3);
@@ -464,35 +390,42 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int u = 0; u < 4; ++u)
               sts128u(tile + (uint32_t)(((u0 + u) ^ sw) << 4), make_uint4(pk[4 * u], pk[4 * u + 1], pk[4 * u + 2], pk[4 * u + 3]));
           }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> tensor core reads
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(mid_ready);
+          fence_proxy_async();              // generic-proxy writes -> tensor core reads
+          named_bar_sync(1, 256);           // intermediate tile complete; every warp is done with the first accumulators
+          // ---- second GEMM: this warpgroup's 64 rows of the intermediate x the resident weight ----
+          mbar_wait(w1_bar, 0);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) accr[i] = 0.f;
+          wgmma_fence();
+#pragma unroll
+          for (int kc = 0; kc < BN / BK; ++kc) {
+            const uint64_t dm = make_kmajor_desc<BK * 2>(smem_u32(s_mid + kc * (GEMM_BM * BK * 2) + wg * 64 * BK * 2));
+            const uint64_t dw = make_kmajor_desc<BK * 2>(smem_u32(s_w1 + kc * (BN * BK * 2)));
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) Wgmma<BN>::ss(accr, dm + (uint64_t)(k * 2), dw + (uint64_t)(k * 2), 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(accr);
+          acc_dump();
+          named_bar_sync(1, 256);
           load_res(half * 32, rr);
-          mbar_wait(&b2b_full[acc], acc_phase);
-          tc_fence_after();
         } else {
           load_res(half * 32, rr);
-          mbar_wait(&tmem_full[acc], acc_phase);
-          tc_fence_after();
         }
 #pragma unroll 1
         for (int c = half * 32; c < BN; c += 64) {
           if (n0 + c >= P.N) break;
           if (c + 64 < BN) load_res(c + 64, rr_n);
           const int n = n0 + c + tr_c;
-          float4 g4[8];                         // gate values: requested before the TMEM read / transpose, used after
+          float4 g4[8];                         // gate values: requested before the accumulator read, used after
           if (!B2B && !kNorm && P.gate) {       // (the codec's back-to-back tiles have no gate: keep their registers)
             const float* g0 = P.gate + n;
 #pragma unroll
             for (int p = 0; p < 8; ++p) g4[p] = __ldg(reinterpret_cast<const float4*>(g0 + item_p[p] * P.gate_ld));
           }
-          float v[32];
-          tmem_ld32(t_addr + c, v);
-          tmem_ld_wait();
-          stage_put(v);
           float4 x[8];
-          stage_get(x);
+          acc_get(c, x);
           if (P.bias) {
             const float4 b4 = __ldg(reinterpret_cast<const float4*>(P.bias + (P.bias_mod ? (n % P.bias_mod) : n)));
 #pragma unroll
@@ -581,15 +514,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       } else if constexpr (MODE == EPI_SWIGLU) {
         // tile columns: [32 gate | 32 up] pairs -> BN/2 outputs at column n0/2; this warp owns alternating pairs
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
 #pragma unroll 1
         for (int c = half * 64; c < BN; c += 128) {
           if (n0 + c >= P.N) break;
           float g[32], u[32];
-          tmem_ld32(t_addr + c, g);
-          tmem_ld32(t_addr + c + 32, u);
-          tmem_ld_wait();
+          acc_ld32(c, g);
+          acc_ld32(c + 32, u);
           if (P.ssq_in) {   // fused RMSNorm: rstd * acc + (shift @ W^T) of this row's item (L1-broadcast loads)
 #pragma unroll
             for (int j = 0; j < 32; j += 4) {
@@ -603,9 +533,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
 #pragma unroll
           for (int j = 0; j < 32; ++j) g[j] = silu_f(g[j]) * u[j];
-          stage_put(g);
+          acc_put(c, g);
           float4 x[8];
-          stage_get(x);
+          acc_get(c, x);
           __nv_bfloat16* o0 = P.out_bf16 + row0 * P.out_bf16_ld + ((n0 + c) >> 1) + tr_c;
           const long long st = 4 * P.out_bf16_ld;
 #pragma unroll
@@ -617,8 +547,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         int pos[8];                             // RoPE position of each pass (one modulo per tile)
 #pragma unroll
         for (int p = 0; p < 8; ++p) pos[p] = (int)(((uint32_t)row0 + 4u * p) % (uint32_t)P.rope_T);   // rows < 2^31: no 64-bit division
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
         constexpr int kHeadStep = (BN >= 256) ? 256 : 128;   // BN=128: both warps of a quarter share the single head
 #pragma unroll 1
         for (int hc = (BN >= 256 ? half * 128 : 0); hc < BN; hc += kHeadStep) {
@@ -641,8 +569,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll 1
             for (int c = 0; c < 128; c += 32) {
               float v[32];
-              tmem_ld32(t_addr + hc + c, v);
-              tmem_ld_wait();
+              acc_ld32(hc + c, v);
 #pragma unroll
               for (int i = 0; i < 32; i += 4) {
                 const float4 w4 = __ldg(reinterpret_cast<const float4*>(nw + c + i));
@@ -712,9 +639,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                   }
                 }
               }
-              stage_put(o);
+              acc_put(hc + c, o);
               float4 x[8];
-              stage_get(x);
+              acc_get(hc + c, x);
               __nv_bfloat16* o0 = P.out_bf16 + row0 * P.out_bf16_ld + nh + c + tr_c;
               const long long st = 4 * P.out_bf16_ld;
 #pragma unroll
@@ -730,8 +657,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll 1
             for (int c = 0; c < 128; c += 32) {
               float v[32];
-              tmem_ld32(t_addr + hc + c, v);
-              tmem_ld_wait();
+              acc_ld32(hc + c, v);
               if (P.ssq_in) {   // fused RMSNorm of the GEMM's input rows: the head's values are rstd * acc + bias
 #pragma unroll
                 for (int j = 0; j < 32; j += 4) {
@@ -759,13 +685,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
 #pragma unroll 1
           for (int c = (BN >= 256 ? 0 : half * 32); c < 128; c += (BN >= 256 ? 32 : 64)) {
-            float v[32];
-            tmem_ld32(t_addr + hc + c, v);
-            tmem_ld_wait();
-            stage_put(v);
             const int cc = c + tr_c;              // column inside the head
             float4 x[8];
-            stage_get(x);
+            acc_get(hc + c, x);
             if (P.ssq_in) {
               const float* b0 = P.ibias + nh + cc;
 #pragma unroll
@@ -800,24 +722,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
-      // release the accumulator back to the MMA warp (on the leader CTA's barrier)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 2) mbar_arrive_cluster(&tmem_empty[acc], 0);
-        else mbar_arrive(&tmem_empty[acc]);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      named_bar_sync(1, 256);   // the accumulator tile may be overwritten by the next tile's main loop
     }
   }
 
-  tc_fence_before();
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_cg2<kTmemCols>(tmem_base);
-    else tmem_dealloc<kTmemCols>(tmem_base);
-  }
 }
 
 }  // namespace sab

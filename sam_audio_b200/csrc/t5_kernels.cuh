@@ -1,6 +1,6 @@
 // Small kernels of the T5 text encoder (reference: sam_audio/model/text_encoder.py:11-37 wraps HF T5EncoderModel;
 // arithmetic = transformers' T5Stack: T5LayerNorm (RMS, eps 1e-6), un-scaled dot-product attention with a
-// bucketed relative position bias, DenseReluDense).  The linears run on the tcgen05 GEMM; text is a handful of
+// bucketed relative position bias, DenseReluDense).  The linears run on the wgmma GEMM; text is a handful of
 // tokens, so these kernels are latency- not throughput-critical.
 #pragma once
 #include "common.cuh"

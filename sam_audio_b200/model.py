@@ -1,13 +1,13 @@
-"""SAMAudio — B200 drop-in for the reference's ``model.separate()`` path.
+"""SAMAudio — H100 drop-in for the reference's ``model.separate()`` path.
 
 Same public surface as the reference class (reference: sam_audio/model/model.py:75-359,
 sam_audio/model/base.py:17-62): ``SAMAudio.from_pretrained``, ``.eval()/.to()/.cuda()``,
 ``.sample_rate``, ``.separate(batch, noise=None, ode_opt=DFLT_ODE_OPT,
 reranking_candidates=1, predict_spans=False) -> SeparationResult``, ``.forward`` (one ODE
 function evaluation), ``.unbatch``.  All arithmetic of the path runs in
-libsamaudio_b200.so (hand-written sm_100a kernels) through the C ABI in
+libsamaudio_b200.so (hand-written sm_90a kernels) through the C ABI in
 include/samaudio_b200.h; this file only moves pointers and mirrors control flow.
-There is no PyTorch / CPU fallback: without the library and a B200 it raises.
+There is no PyTorch / CPU fallback: without the library and an H100 it raises.
 """
 from __future__ import annotations
 
@@ -160,7 +160,7 @@ class SAMAudio(torch.nn.Module):
     def _ensure_engine(self) -> _capi.Engine:
         if self._engine is None:
             if self._device.type != "cuda":
-                raise RuntimeError("sam_audio_b200.SAMAudio runs on a B200 only: call .cuda() first "
+                raise RuntimeError("sam_audio_b200.SAMAudio runs on an H100 only: call .cuda() first "
                                    "(there is no CPU path)")
             if self._state is None:
                 raise RuntimeError("no weights loaded: call load_state_dict()/from_pretrained() first")

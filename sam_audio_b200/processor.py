@@ -119,7 +119,7 @@ def load_video(sizes, videos, feature_idx_to_wav_idx, audio_sampling_rate):
     picked = []
     for size, video in zip(sizes, videos):
         if isinstance(video, str):
-            raise NotImplementedError("video file decoding (torchcodec) is outside the B200 hot path; pass tensors")
+            raise NotImplementedError("video file decoding (torchcodec) is outside the H100 hot path; pass tensors")
         assert video.size(1) == 3, f"expected NCHW video, found {video.size(1)} channels"
         idx = torch.linspace(0, video.size(0) - 1, int(size)).round().long()
         picked.append(video[idx])
@@ -161,7 +161,7 @@ class Processor:
         out = []
         for v, m in zip(videos, masks):
             if isinstance(v, str) or isinstance(m, str):
-                raise NotImplementedError("video file decoding (torchcodec) is outside the B200 hot path; pass tensors")
+                raise NotImplementedError("video file decoding (torchcodec) is outside the H100 hot path; pass tensors")
             out.append(v * m.eq(0))
         return out
 

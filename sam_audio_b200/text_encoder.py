@@ -1,9 +1,9 @@
 """Text conditioning: T5 encoder wrapper (reference: sam_audio/model/text_encoder.py:11-37).
 
-Tokenisation stays on the host (HF tokenizer); on a B200 the encoder stack itself
+Tokenisation stays on the host (HF tokenizer); on an H100 the encoder stack itself
 runs natively through ``sab_t5_forward`` (SURVEY.md §8a a5 / §8f-3 "next" row:
 T5LayerNorm, un-scaled attention with the bucketed relative-position bias and
-DenseReluDense on the same tcgen05 GEMM as the DiT), checked against
+DenseReluDense on the same wgmma GEMM as the DiT), checked against
 ``transformers.T5EncoderModel`` in tests/test_gpu_parity.py.  The HF module is kept
 only as the weight container (``from_pretrained`` / ``state_dict``); its forward is never called here.  When no ``t5-base``
 checkpoint/tokenizer is on disk (this sandbox has no network) the same module
@@ -118,7 +118,7 @@ class T5TextEncoder(torch.nn.Module):
         input_ids = enc["input_ids"].to(device)
         attention_mask = enc["attention_mask"].to(device)
         if device.type != "cuda":
-            raise RuntimeError("T5TextEncoder runs on a B200 only: move the model to cuda first (no CPU path)")
+            raise RuntimeError("T5TextEncoder runs on an H100 only: move the model to cuda first (no CPU path)")
         B, L = input_ids.shape
         eng = self._engine(device)
         cfg = self.model.config

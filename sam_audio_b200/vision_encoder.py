@@ -2,7 +2,7 @@
 (reference: sam_audio/model/vision_encoder.py:16-113).
 
 What is built natively: the frame pre-processing (`get_transform`: antialiased bicubic resize to image_size^2 on uint8
-frames, /255, Normalize(.5,.5)) as sm_100a kernels behind `sab_preprocess_frames`, and the control flow of
+frames, /255, Normalize(.5,.5)) as sm_90a kernels behind `sab_preprocess_frames`, and the control flow of
 `VisionEncoder.forward` (per-video transform, chunks of `batch_size` frames, zero pad_sequence).  What is NOT here: the
 PE-Core-L14-336 CLIP tower itself (third-party `perception-models`, source and weights absent — SURVEY §8f-2): pass it as
 `model` (anything with `encode_image(x, normalize=...)`); without one, encoding raises.
@@ -22,7 +22,7 @@ class PerceptionEncoder(torch.nn.Module):
         super().__init__()
         cfg = cfg or PerceptionEncoderConfig()
         if cfg.interpolation_mode.upper() != "BICUBIC":
-            raise NotImplementedError(f"interpolation_mode {cfg.interpolation_mode!r}: the B200 kernel implements the "
+            raise NotImplementedError(f"interpolation_mode {cfg.interpolation_mode!r}: the H100 kernel implements the "
                                       "reference's shipped BICUBIC (antialiased) resize")
         self.batch_size = cfg.batch_size
         self.dim = cfg.dim
@@ -34,10 +34,10 @@ class PerceptionEncoder(torch.nn.Module):
     def transform(self, video: torch.Tensor) -> torch.Tensor:
         """[T, 3, H, W] uint8 -> [T, 3, S, S] float32 on the video's (cuda) device — vision_encoder.py:91-113."""
         if video.dtype != torch.uint8:
-            raise NotImplementedError("the reference pipeline feeds uint8 frames (torchcodec / mask_videos); the B200 "
+            raise NotImplementedError("the reference pipeline feeds uint8 frames (torchcodec / mask_videos); the H100 "
                                       "resize kernel reproduces torchvision's uint8 rounding")
         if not video.is_cuda:
-            raise RuntimeError("PerceptionEncoder.transform runs on a B200 only: move the frames to cuda (no CPU path)")
+            raise RuntimeError("PerceptionEncoder.transform runs on an H100 only: move the frames to cuda (no CPU path)")
         return _capi.preprocess_frames(video, self.image_size)
 
     def encode(self, x: torch.Tensor) -> torch.Tensor:

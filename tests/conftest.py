@@ -31,7 +31,7 @@ def usable_host_cores() -> int:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (select with -m gpu)")
     import torch
     torch.set_num_threads(usable_host_cores())
 

@@ -1,4 +1,4 @@
-"""GPU (B200) parity tests — the CUDA path, called through the C ABI (ctypes) and the public Python
+"""GPU (H100) parity tests — the CUDA path, called through the C ABI (ctypes) and the public Python
 mirror, against (a) golden vectors produced by the reference's own code, (b) the CPU oracle on the same
 seeded inputs, and (c) size-independent properties at the full 10 s / 48 kHz clip size.
 
@@ -15,7 +15,7 @@ import os
 import pytest
 import torch
 
-from _util import rel_l2, snr_db
+from _util import load_golden, rel_l2, snr_db
 
 pytestmark = pytest.mark.gpu
 
@@ -33,7 +33,7 @@ def capi():
     (128, 256, 64, 256, 64, 1), (300, 256, 256, 256, 64, 1), (1000, 512, 2048, 128, 64, 1),
     (2500, 2048, 2048, 256, 64, 1), (300, 96, 96, 96, 32, 1), (777, 128, 160, 128, 32, 1),
     (500, 192, 192, 192, 64, 1), (333, 96, 192, 96, 64, 1), (129, 64, 128, 64, 64, 1), (1, 256, 64, 256, 64, 1),
-    # cta_group::2 pairs (256-row tiles)
+    # 2-CTA clusters (256-row tiles, B tile multicast to both CTAs)
     (256, 256, 64, 256, 64, 2), (300, 512, 256, 256, 64, 2), (2500, 2048, 2048, 256, 64, 2),
     (16000, 2816, 2816, 256, 64, 2), (100, 256, 128, 256, 64, 2), (5000, 11008, 512, 256, 64, 0)])
 def test_tcgen05_gemm(capi, M, N, K, bn, bk, cg):
@@ -65,32 +65,13 @@ def test_attention(capi, items, heads, Tq, Tk):
     assert rel_l2(o.float(), ref) < 1e-2
 
 
-@pytest.mark.parametrize("items,heads,T", [(1, 1, 256), (2, 3, 250), (3, 2, 37), (2, 2, 129), (1, 1, 1), (2, 1, 128)])
-def test_tcgen05_self_attention(capi, items, heads, T):
-    """TMA + tcgen05 QK^T / in-TMEM softmax / TS-form PV kernel (T <= 256) vs fp32 torch, ragged key masks."""
-    g = torch.Generator(device="cuda").manual_seed(T + items)
-    q, k, v = (torch.randn(items * T, heads * 128, device="cuda", generator=g).bfloat16() for _ in range(3))
-    mask = torch.ones(items, T, dtype=torch.uint8, device="cuda")
-    for i in range(items):
-        mask[i, max(1, T - 3 * (i + 1)):] = 0
-    o = torch.zeros(items * T, heads * 128, device="cuda", dtype=torch.bfloat16)
-    capi.check(capi.lib().sab_test_attention_tc(items, heads, T, q.data_ptr(), k.data_ptr(), v.data_ptr(),
-                                                mask.data_ptr(), o.data_ptr(), 0, 0, capi.stream_ptr()))
-    torch.cuda.synchronize()
-    qf, kf, vf = (x.float().view(items, T, heads, 128).permute(0, 2, 1, 3) for x in (q, k, v))
-    s = (qf @ kf.transpose(-1, -2) / 128 ** 0.5).masked_fill(~mask.bool()[:, None, None, :], float("-inf"))
-    ref = (torch.softmax(s, -1) @ vf).permute(0, 2, 1, 3).reshape(items * T, heads * 128)
-    assert rel_l2(o.float(), ref) < 1e-2
-
-
 @pytest.mark.parametrize("exact", [False, True])
 @pytest.mark.parametrize("items,heads,T", [(1, 1, 256), (2, 3, 250), (3, 2, 37), (2, 2, 129), (1, 1, 1), (2, 1, 128),
                                            (40, 8, 250), (37, 5, 131)])
 def test_tcgen05_self_attention_v2(capi, items, heads, T, exact):
-    """Second-generation kernel (attention_tc2.cuh): 16 softmax warps, P/O per key half in TMEM, TMA-stored output;
-    exact = two-pass row maximum, otherwise the single-pass softmax with a logit bound (here the Cauchy-Schwarz bound
-    of the actual q, k); polynomial exp2 on 3 of 8 pairs.  The last two shapes give every persistent CTA several work
-    items (the cross-item pipeline: prefetch, TMEM hand-over, staging-tile hand-over)."""
+    """wgmma self-attention kernel (attention_tc2.cuh; T <= 256) vs fp32 torch, ragged key masks: exact = two-pass
+    row maximum, otherwise the single-pass softmax with a logit bound (here the Cauchy-Schwarz bound of the actual
+    q, k); polynomial exp2 on 3 of 8 pairs or none.  The last two shapes run many (item, head) CTAs per SM."""
     g = torch.Generator(device="cuda").manual_seed(T + items)
     q, k, v = (torch.randn(items * T, heads * 128, device="cuda", generator=g).bfloat16() for _ in range(3))
     mask = torch.ones(items, T, dtype=torch.uint8, device="cuda")
@@ -106,7 +87,7 @@ def test_tcgen05_self_attention_v2(capi, items, heads, T, exact):
     for poly in (3, 0):
         o.fill_(float("nan"))
         capi.check(capi.lib().sab_test_attention_tc2(items, heads, T, q.data_ptr(), k.data_ptr(), v.data_ptr(),
-                                                     mask.data_ptr(), o.data_ptr(), shift, poly, None, capi.stream_ptr()))
+                                                     mask.data_ptr(), o.data_ptr(), shift, poly, capi.stream_ptr()))
         torch.cuda.synchronize()
         assert not torch.isnan(o.float()).any()
         assert rel_l2(o.float(), ref) < 1e-2, (poly, exact)
@@ -120,14 +101,14 @@ def test_tcgen05_self_attention_v2(capi, items, heads, T, exact):
         ref2 = ref2.permute(0, 2, 1, 3).reshape(items * T, heads * 128)
         o.fill_(float("nan"))
         capi.check(capi.lib().sab_test_attention_tc2(items, heads, T, qs.data_ptr(), k.data_ptr(), v.data_ptr(),
-                                                     mask.data_ptr(), o.data_ptr(), 0.0, 3, None, capi.stream_ptr()))
+                                                     mask.data_ptr(), o.data_ptr(), 0.0, 3, capi.stream_ptr()))
         torch.cuda.synchronize()
         assert not torch.isnan(o.float()).any()
         assert rel_l2(o.float(), ref2) < 1e-2
 
 
 def test_long_sequence_uses_streaming_attention(tiny_model):
-    """T > 256 frames (a 12 s clip) falls back from the single-pass tcgen05 kernel to the streaming one;
+    """T > 256 frames (a 12 s clip) falls back from the single-pass wgmma kernel to the streaming one;
     the result must agree with the same clip's first 10 s only in shape/finite-ness (different content),
     and batch invariance must still hold."""
     from sam_audio_b200 import SAMAudioProcessor
@@ -144,7 +125,7 @@ def test_long_sequence_uses_streaming_attention(tiny_model):
 def test_dit_evaluation_vs_reference_golden(tiny_model, golden_dir):
     """SAMAudio.forward (ragged pad mask, text mask, anchors, with and without video) vs the reference's
     own SAMAudio.forward output (tests/golden/samaudio_forward_tiny.pt)."""
-    g = torch.load(os.path.join(golden_dir, "samaudio_forward_tiny.pt"))
+    g = load_golden(golden_dir, "samaudio_forward_tiny")
     for tag, vid in (("video", g["video"]), ("novideo", torch.zeros_like(g["video"]))):
         out = tiny_model.forward(g["noisy"].cuda(), g["feats"].cuda(), g["text"].cuda(), g["time"].cuda(),
                                  masked_video_features=vid.cuda(),
@@ -156,7 +137,7 @@ def test_dit_evaluation_vs_reference_golden(tiny_model, golden_dir):
 def test_dit_evaluation_none_arguments_vs_reference_golden(tiny_model, golden_dir):
     """The `None` cases of SAMAudio.forward mean what they mean in the reference: no video term (align.py:41-42),
     no anchor term (model.py:57-58), time-only memory (model.py:170-172) — golden = the reference's own output."""
-    g = torch.load(os.path.join(golden_dir, "samaudio_forward_tiny.pt"))
+    g = load_golden(golden_dir, "samaudio_forward_tiny")
     out = tiny_model.forward(g["noisy"].cuda(), g["feats"].cuda(), g["text"].cuda(), g["time"].cuda(),
                              text_mask=g["text_mask"].cuda(), audio_pad_mask=g["pad_mask"].cuda())
     assert rel_l2(out.cpu(), g["out"]["none_video_anchors"]) < 2e-2
@@ -191,7 +172,7 @@ def test_dit_evaluation_text_lengths_vs_oracle(tiny_model, tiny_cfg, tiny_sd, L)
 
 @pytest.fixture(scope="module")
 def small_model_and_sd():
-    """sam-audio-small stand-in (d=1536, 12 layers, 12 heads): production tile shapes, 2-CTA GEMMs, T=250."""
+    """sam-audio-small stand-in (d=1536, 12 layers, 12 heads): production tile shapes, 2-CTA cluster GEMMs, T=250."""
     from sam_audio_b200.config import stand_in_config
     from sam_audio_b200.model import SAMAudio
     from sam_audio_b200.synthetic import make_state_dict
@@ -204,8 +185,8 @@ def small_model_and_sd():
 
 
 def test_dit_evaluation_production_shapes_vs_oracle(small_model_and_sd):
-    """One ODE function evaluation at production width and clip length (B=5 x T=250 -> M=1250 rows: cta_group::2 GEMM
-    pairs, tcgen05 self-attention, fused text cross-attention) vs the fp32 CPU oracle."""
+    """One ODE function evaluation at production width and clip length (B=5 x T=250 -> M=1250 rows: 2-CTA cluster
+    GEMMs, wgmma self-attention, fused text cross-attention) vs the fp32 CPU oracle."""
     from oracle import restate
     m, cfg, sd = small_model_and_sd
     g = torch.Generator().manual_seed(5)
@@ -246,7 +227,7 @@ def test_separate_full_clip_size_vs_oracle(small_model_and_sd):
 
 
 def test_native_t5_encoder_vs_transformers(capi):
-    """sab_t5_forward (tcgen05 GEMMs + relative-bias attention) vs transformers.T5EncoderModel with the same
+    """sab_t5_forward (wgmma GEMMs + relative-bias attention) vs transformers.T5EncoderModel with the same
     random t5-base-shaped weights, ragged descriptions (padding mask) — tolerance as for one DiT evaluation."""
     from sam_audio_b200.config import T5EncoderConfig
     from sam_audio_b200.text_encoder import T5TextEncoder, t5_relative_buckets
@@ -290,7 +271,7 @@ def test_separate_vs_reference_golden(tiny_model, golden_dir, cand):
     conditioning inside the engine instead of the reference's expand/reshape copies, model.py:193-203)."""
     from sam_audio_b200 import SAMAudioProcessor
     from sam_audio_b200.synthetic import synthetic_clip, synthetic_descriptions
-    g = torch.load(os.path.join(golden_dir, "separate_tiny.pt"))
+    g = load_golden(golden_dir, "separate_tiny")
     proc = SAMAudioProcessor(1920, 48000)
     auds = [synthetic_clip(i, n) for i, n in enumerate(g["lens"])]
     batch = proc(descriptions=synthetic_descriptions(2), audios=auds).to("cuda")
@@ -327,7 +308,7 @@ def test_candidate_selection_through_attached_rankers_vs_reference_golden(tiny_m
     from sam_audio_b200 import SAMAudioProcessor
     from sam_audio_b200.ranking import EnsembleRanker
     from sam_audio_b200.synthetic import synthetic_clip, synthetic_descriptions
-    g = torch.load(os.path.join(golden_dir, "separate_tiny.pt"))
+    g = load_golden(golden_dir, "separate_tiny")
     r = g["results"]["ranked3"]
     proc = SAMAudioProcessor(1920, 48000)
     auds = [synthetic_clip(i, n) for i, n in enumerate(g["lens"])]
@@ -462,7 +443,7 @@ def test_solver_composition_and_determinism(tiny_model):
 
 def test_exact_softmax_fallback_and_many_anchor_ids(tiny_cfg, tiny_sd, golden_dir, monkeypatch):
     """(1) Layers whose QK-norm weights do not bound the logits tightly enough run the exact two-pass softmax variant of
-    the tcgen05 attention kernel (forced here through SAB_ATTN_EXACT): same golden as the single-pass path.
+    the wgmma attention kernel (forced here through SAB_ATTN_EXACT): same golden as the single-pass path.
     (2) More anchor ids per clip than the plan's initial table (64) rebuild the plan instead of failing."""
     from oracle import restate
     from sam_audio_b200.model import SAMAudio
@@ -473,7 +454,7 @@ def test_exact_softmax_fallback_and_many_anchor_ids(tiny_cfg, tiny_sd, golden_di
     m = m.eval().cuda()
     m._ensure_engine()                                     # the env is read when the weights are finalised
     monkeypatch.delenv("SAB_ATTN_EXACT")
-    g = torch.load(os.path.join(golden_dir, "samaudio_forward_tiny.pt"))
+    g = load_golden(golden_dir, "samaudio_forward_tiny")
     out = m.forward(g["noisy"].cuda(), g["feats"].cuda(), g["text"].cuda(), g["time"].cuda(),
                     masked_video_features=g["video"].cuda(), text_mask=g["text_mask"].cuda(),
                     anchor_ids=g["anchor_ids"].cuda(), anchor_alignment=g["anchor_alignment"].cuda(),
@@ -522,7 +503,7 @@ def test_missing_or_unknown_weights_fail_loudly(tiny_cfg, tiny_sd):
     assert res.unexpected_keys == ["transformer.bogus.weight"] and res.missing_keys == ["audio_codec.decoder.model.0.bias"]
     m3 = SAMAudio(tiny_cfg, text_encoder=SyntheticTextEncoder())
     m3.load_state_dict(tiny_sd)
-    with pytest.raises(RuntimeError, match="B200 only"):
+    with pytest.raises(RuntimeError, match="H100 only"):
         m3._ensure_engine()                                  # still on CPU: no fallback
 
 

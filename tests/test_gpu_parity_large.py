@@ -1,4 +1,4 @@
-"""GPU (B200) parity at the BENCHMARKED shapes — sam-audio-large (d 2816 / 22 heads / 24 layers) and sam-audio-small —
+"""GPU (H100) parity at the BENCHMARKED shapes — sam-audio-large (d 2816 / 22 heads / 24 layers) and sam-audio-small —
 against the fp32 CPU oracle: one ODE function evaluation at T = 250 with ragged masks, the full 32-evaluation
 separate() of a 10 s @ 48 kHz clip (error compounding at production depth x length), and batch invariance of a clip
 inside the B = 64 batch bench.py times.
@@ -92,7 +92,7 @@ def test_large_full_32_evaluations_vs_oracle(large):
 
 def test_large_batch_invariance_b64(large):
     """Clip 0 separated alone == clip 0 inside the B = 64 batch that bench.py times (every op is per sequence; the
-    GEMM tiles, cta_group::2 pairs and codec chunks it lands in differ)."""
+    GEMM tiles, 2-CTA clusters and codec chunks it lands in differ)."""
     m = large[0]
     from sam_audio_b200 import SAMAudioProcessor
     from sam_audio_b200.synthetic import synthetic_clip, synthetic_descriptions, synthetic_noise

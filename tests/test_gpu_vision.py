@@ -1,4 +1,4 @@
-"""GPU (B200): visual-prompting front end — the frame pre-processing kernels (sab_preprocess_frames) against the oracle
+"""GPU (H100): visual-prompting front end — the frame pre-processing kernels (sab_preprocess_frames) against the oracle
 restatement (pinned to torchvision, tests/test_oracle_vision.py), the PerceptionEncoder mirror's chunked encode against the
 golden output of the reference's own class, and config-5-style separate() with masked video through a stand-in tower."""
 import os

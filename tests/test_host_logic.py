@@ -100,7 +100,7 @@ def test_from_pretrained_local_directory_and_no_cpu_path(tmp_path):
     proc = SAMAudioProcessor.from_pretrained(str(tmp_path))
     assert proc.audio_hop_length == 1920 and proc.audio_sampling_rate == 48000
     batch = proc(descriptions=["thunder"], audios=[torch.zeros(1, 4000)])
-    with pytest.raises(RuntimeError, match="B200 only"):
+    with pytest.raises(RuntimeError, match="H100 only"):
         m.eval().separate(batch)
 
 
@@ -132,7 +132,7 @@ def test_separate_validates_ode_opt_before_touching_the_gpu():
     for bad in ({"method": "dopri5"}, {"method": "midpoint"}, {"method": "rk4", "options": {"step_size": 0.3}}):
         with pytest.raises(NotImplementedError):
             m.separate(None, ode_opt=bad)
-    with pytest.raises(RuntimeError, match="B200 only|no weights"):      # valid options: next stop is the (absent) engine
+    with pytest.raises(RuntimeError, match="H100 only|no weights"):      # valid options: next stop is the (absent) engine
         m.separate(None, ode_opt={"method": "euler", "options": {"step_size": 0.125}})
 
 
@@ -166,7 +166,7 @@ def test_perception_encoder_wrapper_host_behaviour():
     from sam_audio_b200.vision_encoder import PerceptionEncoder
     enc = PerceptionEncoder(PerceptionEncoderConfig())
     assert enc.batch_size == 300 and enc.image_size == 336 and enc.dim == 1024
-    with pytest.raises(RuntimeError, match="B200 only"):
+    with pytest.raises(RuntimeError, match="H100 only"):
         enc.transform(torch.zeros(2, 3, 8, 8, dtype=torch.uint8))            # no CPU path
     with pytest.raises(NotImplementedError):
         enc.transform(torch.zeros(2, 3, 8, 8))                               # the reference feeds uint8 frames

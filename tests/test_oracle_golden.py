@@ -6,7 +6,7 @@ import torch
 
 from oracle import restate
 from sam_audio_b200 import synthetic
-from _util import rel_l2
+from _util import load_golden, rel_l2
 
 torch.set_grad_enabled(False)
 
@@ -19,7 +19,7 @@ def test_dit_forward_matches_reference_golden(golden_dir, tiny_cfg, tiny_sd):
 
 
 def test_samaudio_forward_matches_reference_golden(golden_dir, tiny_cfg, tiny_sd):
-    g = torch.load(os.path.join(golden_dir, "samaudio_forward_tiny.pt"))
+    g = load_golden(golden_dir, "samaudio_forward_tiny")
     for tag, vid in (("video", g["video"]), ("novideo", torch.zeros_like(g["video"]))):
         out = restate.samaudio_forward(tiny_sd, tiny_cfg, g["noisy"], g["feats"], g["text"], g["time"], vid,
                                        g["text_mask"], g["anchor_ids"], g["anchor_alignment"], g["pad_mask"])
@@ -77,7 +77,7 @@ def test_other_fixed_grid_solvers_orders_of_accuracy():
 
 def test_separate_control_flow_matches_reference_golden(golden_dir, tiny_cfg, tiny_sd):
     """encode -> 32 evaluations -> decode -> unbatch, candidates 1 and 8 (reference pipeline output)."""
-    g = torch.load(os.path.join(golden_dir, "separate_tiny.pt"))
+    g = load_golden(golden_dir, "separate_tiny")
     auds = [synthetic.synthetic_clip(i, n) for i, n in enumerate(g["lens"])]
     aud, ws = restate.batch_audio(auds)
     sizes = restate.wav_to_feature_idx(ws, 1920)
@@ -95,7 +95,7 @@ def test_separate_control_flow_matches_reference_golden(golden_dir, tiny_cfg, ti
 
 def test_ranked_candidate_selection_matches_reference_golden(golden_dir, tiny_cfg, tiny_sd):
     """model.py:306-330 with an attached (stand-in, fixed-score) text ranker: arg-max candidate per clip."""
-    g = torch.load(os.path.join(golden_dir, "separate_tiny.pt"))
+    g = load_golden(golden_dir, "separate_tiny")
     r = g["results"]["ranked3"]
     auds = [synthetic.synthetic_clip(i, n) for i, n in enumerate(g["lens"])]
     aud, ws = restate.batch_audio(auds)
