@@ -579,7 +579,7 @@ struct DitPlan {
   int64_t M = 0, MB = 0, ML = 0;        // sequence rows Bc*T, clip rows B*T, clip text rows B*L
   float* condB = nullptr;               // clip-level conditioning GEMM output (aliases cond when cand == 1)
   // fused RMSNorm + modulate (gemm_tc.cuh): column scales w*(1+scale) [2NL, Bc, d], bf16 shifts [2NL, Bc, d],
-  // per-(row, n-tile, warp half) partial sums of squares [M, ssq_n], per-item biases shift @ W^T
+  // per-(row, n-tile, 32-column chunk parity) partial sums of squares [M, ssq_n], per-item biases shift @ W^T
   bool fused_norm = false;
   float* nrm_ssq = nullptr;
   int ssq_n = 0;
