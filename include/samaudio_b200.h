@@ -151,6 +151,55 @@ int64_t sab_t5_launch_count(sab_t5* e, int reset);
  * 128-row tile, cg = 2: 2-CTA clusters on 256-row tiles sharing the B tile, cg = 0: the engine's default choice). */
 int sab_test_gemm(int M, int N, int K, const void* a_bf16, const void* b_bf16, float* c, int bn, int bk, int cg,
                   void* stream);
+
+/* The whole GEMM contract (sam_audio_b200/csrc/gemm_tc.cuh): one launch planned by the engine's own planner
+ * (tile counts, TMA maps, cluster choice) with every epilogue field of GemmParams under the caller's control.
+ * The descriptor and the epilogue combination are checked by the same rules as every engine plan, before any CUDA
+ * call; a rejected descriptor returns non-zero with the rule in sab_last_error(). */
+typedef struct sab_test_gemm_run {
+  int32_t row_shift;  /* added to the tile's first row; rows outside [0, a_rows) read as zero */
+  int32_t a_col;      /* first A column of the run */
+  int32_t nkb;        /* number of bk-wide k-blocks */
+} sab_test_gemm_run;
+typedef struct sab_test_gemm_desc {
+  int32_t struct_bytes;     /* = sizeof(sab_test_gemm_desc), checked first */
+  /* tile */
+  int32_t mode;             /* 0 affine, 1 SwiGLU, 2 QKV, 3 affine + fused-RMSNorm producer */
+  int32_t bn, bk, cg, b2b;  /* cg = 0: the engine's choice; b2b: back-to-back second GEMM (codec residual unit) */
+  /* A (bf16): a_cols visible columns, a_rows rows per item, a_items items; pitches in elements (0: packed) */
+  const void* a;
+  int64_t a_cols, a_rows, a_items, a_row_pitch, a_item_pitch;
+  /* B (bf16) [n, sum of the run list's k-blocks * bk], K-major; w1: the b2b second weight [n, n] */
+  const void* b;
+  int32_t n;
+  const void* w1;
+  /* K runs: list 1 applies to the n-tiles with n_period > 0 and (n0 % n_period) >= n_switch */
+  int32_t n_runs[2];
+  sab_test_gemm_run runs[2][8];
+  int32_t n_period, n_switch;
+  /* schedule overrides, 0 = the engine's default */
+  int32_t grid_ctas, group_m, reverse_m;
+  /* epilogue: the GemmParams fields of the same names, with the same meaning */
+  const float* bias; int32_t bias_mod;
+  const float* gate; int32_t gate_ld, gate_div;
+  float alpha; int32_t relu;
+  const float* res; int64_t res_ld;
+  float* out_f32; int64_t out_f32_ld;
+  void* out_bf16; int64_t out_bf16_ld;
+  void* out_act; int64_t out_act_ld; const float* snake_alpha;
+  const float* colscale; int64_t colscale_ld;
+  void* out_scaled; int64_t out_scaled_ld;
+  float* ssq_out; int32_t ssq_ld;
+  const float* ssq_in; int32_t ssq_n; float ssq_inv_dim;
+  const float* ibias; int64_t ibias_ld; int32_t ibias_div;
+  const float* b2b_bias; const float* b2b_alpha;
+  const float* qnorm_w; const float* knorm_w;
+  int32_t n_q_end, n_k_end, qkv_period, norm_w_stride;
+  const void* rope; int32_t rope_T, use_rope; float eps;   /* rope: [rope_T, 64] (cos, sin) float pairs */
+  const void* xa_kv; int64_t xa_kv_ld; int32_t xa_v_col0, xa_Tk, xa_T;
+  const uint8_t* xa_mask; float xa_scale_log2;
+} sab_test_gemm_desc;
+int sab_test_gemm_ex(const sab_test_gemm_desc* d, void* stream);
 /* O = softmax(Q K^T / sqrt(128) + mask) V through the attention kernel; all [items*T, heads*128] bf16. */
 int sab_test_attention(int items, int heads, int Tq, int Tk, const void* q, const void* k, const void* v,
                        const uint8_t* key_mask, void* o, void* stream);

@@ -36,10 +36,52 @@ class SabT5Config(ctypes.Structure):
                 ("n_buckets", ctypes.c_int32), ("eps", ctypes.c_float)]
 
 
+class SabTestGemmRun(ctypes.Structure):
+    _fields_ = [("row_shift", ctypes.c_int32), ("a_col", ctypes.c_int32), ("nkb", ctypes.c_int32)]
+
+
+class SabTestGemmDesc(ctypes.Structure):
+    """Mirror of sab_test_gemm_desc (include/samaudio_b200.h); pointers are device addresses as ints."""
+    _i32, _i64, _f32, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p
+    _fields_ = [
+        ("struct_bytes", _i32),
+        ("mode", _i32), ("bn", _i32), ("bk", _i32), ("cg", _i32), ("b2b", _i32),
+        ("a", _vp), ("a_cols", _i64), ("a_rows", _i64), ("a_items", _i64), ("a_row_pitch", _i64), ("a_item_pitch", _i64),
+        ("b", _vp), ("n", _i32), ("w1", _vp),
+        ("n_runs", _i32 * 2), ("runs", (SabTestGemmRun * 8) * 2), ("n_period", _i32), ("n_switch", _i32),
+        ("grid_ctas", _i32), ("group_m", _i32), ("reverse_m", _i32),
+        ("bias", _vp), ("bias_mod", _i32),
+        ("gate", _vp), ("gate_ld", _i32), ("gate_div", _i32),
+        ("alpha", _f32), ("relu", _i32),
+        ("res", _vp), ("res_ld", _i64),
+        ("out_f32", _vp), ("out_f32_ld", _i64),
+        ("out_bf16", _vp), ("out_bf16_ld", _i64),
+        ("out_act", _vp), ("out_act_ld", _i64), ("snake_alpha", _vp),
+        ("colscale", _vp), ("colscale_ld", _i64),
+        ("out_scaled", _vp), ("out_scaled_ld", _i64),
+        ("ssq_out", _vp), ("ssq_ld", _i32),
+        ("ssq_in", _vp), ("ssq_n", _i32), ("ssq_inv_dim", _f32),
+        ("ibias", _vp), ("ibias_ld", _i64), ("ibias_div", _i32),
+        ("b2b_bias", _vp), ("b2b_alpha", _vp),
+        ("qnorm_w", _vp), ("knorm_w", _vp),
+        ("n_q_end", _i32), ("n_k_end", _i32), ("qkv_period", _i32), ("norm_w_stride", _i32),
+        ("rope", _vp), ("rope_T", _i32), ("use_rope", _i32), ("eps", _f32),
+        ("xa_kv", _vp), ("xa_kv_ld", _i64), ("xa_v_col0", _i32), ("xa_Tk", _i32), ("xa_T", _i32),
+        ("xa_mask", _vp), ("xa_scale_log2", _f32),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__()
+        self.struct_bytes = ctypes.sizeof(SabTestGemmDesc)
+        self.alpha, self.gate_div, self.ibias_div, self.eps = 1.0, 1, 1, 1e-5   # the planner's defaults
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
-    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_attention", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_attention", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -75,6 +117,7 @@ def lib() -> ctypes.CDLL:
         L.sab_profile.argtypes = [vp, i32, vp]
         L.sab_profile_report.argtypes = [vp, ctypes.c_char_p, i64, vp]
         L.sab_test_gemm.argtypes = [i32, i32, i32, vp, vp, vp, i32, i32, i32, vp]
+        L.sab_test_gemm_ex.argtypes = [ctypes.POINTER(SabTestGemmDesc), vp]
         L.sab_test_attention.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
         L.sab_test_attention_tc2.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp]
         L.sab_preprocess_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]

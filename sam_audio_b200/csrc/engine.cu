@@ -92,15 +92,18 @@ static void launch_gemm_inst(const GemmOp& op, cudaStream_t st) {
   SAB_CUDA(cudaGetLastError());
 }
 
-static void launch_gemm(const GemmOp& op, cudaStream_t st) {
-  if (op.b2b) {
-    if (op.BN == 64 && op.BK == 64) return launch_gemm_inst<64, 64, EPI_AFFINE, 1, true>(op, st);
-    if (op.BN == 96 && op.BK == 32) return launch_gemm_inst<96, 32, EPI_AFFINE, 1, true>(op, st);
-    if (op.BN == 128 && op.BK == 64) return launch_gemm_inst<128, 64, EPI_AFFINE, 1, true>(op, st);
-    throw Error(fmt("no back-to-back GEMM instantiation for BN=%d BK=%d (%s)", op.BN, op.BK, op.tag));
+// the instantiation table: the launcher of (BN, BK, mode, cg, b2b), or nullptr if that combination is not built
+typedef void (*GemmLauncher)(const GemmOp&, cudaStream_t);
+static GemmLauncher gemm_launcher(int BN, int BK, int mode, int cg, bool b2b) {
+  if (b2b) {
+    if (mode != EPI_AFFINE || cg != 1) return nullptr;
+    if (BN == 64 && BK == 64) return launch_gemm_inst<64, 64, EPI_AFFINE, 1, true>;
+    if (BN == 96 && BK == 32) return launch_gemm_inst<96, 32, EPI_AFFINE, 1, true>;
+    if (BN == 128 && BK == 64) return launch_gemm_inst<128, 64, EPI_AFFINE, 1, true>;
+    return nullptr;
   }
 #define SAB_CASE(bn_, bk_, md_, cg_) \
-  if (op.BN == bn_ && op.BK == bk_ && op.mode == md_ && op.cg == cg_) return launch_gemm_inst<bn_, bk_, md_, cg_>(op, st);
+  if (BN == bn_ && BK == bk_ && mode == md_ && cg == cg_) return launch_gemm_inst<bn_, bk_, md_, cg_>;
   SAB_CASE(256, 64, EPI_AFFINE, 2)
   SAB_CASE(256, 64, EPI_AFFINE_NORM, 2)
   SAB_CASE(256, 64, EPI_AFFINE_NORM, 1)
@@ -117,7 +120,72 @@ static void launch_gemm(const GemmOp& op, cudaStream_t st) {
   SAB_CASE(256, 64, EPI_QKV, 1)
   SAB_CASE(128, 64, EPI_QKV, 1)
 #undef SAB_CASE
-  throw Error(fmt("no GEMM instantiation for BN=%d BK=%d mode=%d cg=%d (%s)", op.BN, op.BK, op.mode, op.cg, op.tag));
+  return nullptr;
+}
+
+// Parameter combinations that the kernel would ignore, or turn into wrong results or stray reads, without an error
+// (beyond what the instantiations' static_asserts cover).  Every launch is checked; host-only (no CUDA call), so the
+// test seam can check a descriptor before it touches the device.
+static void check_gemm(const char* tag, int BN, int BK, int mode, int cg, bool b2b, int grid, const GemmParams& P) {
+  const bool affine = (mode == EPI_AFFINE || mode == EPI_AFFINE_NORM);
+  SAB_CHECK(mode >= EPI_AFFINE && mode <= EPI_AFFINE_NORM, "%s: unknown GEMM mode %d", tag, mode);
+  SAB_CHECK(P.N > 0 && P.N % 32 == 0, "%s: N=%d must be a positive multiple of 32", tag, P.N);
+  SAB_CHECK(mode != EPI_QKV || P.N % 128 == 0, "%s: QKV mode needs whole 128-column heads (N=%d)", tag, P.N);
+  SAB_CHECK(mode != EPI_SWIGLU || P.N % 64 == 0, "%s: SwiGLU mode needs whole [32 gate | 32 up] pairs (N=%d)", tag, P.N);
+  SAB_CHECK(affine || P.out_bf16, "%s: SwiGLU / QKV modes write out_bf16, which is not set", tag);
+  SAB_CHECK(!P.out_act || P.snake_alpha, "%s: out_act needs snake_alpha", tag);
+  SAB_CHECK(mode == EPI_AFFINE_NORM || (!P.out_scaled && !P.ssq_out),
+            "%s: the fused-norm producer outputs (out_scaled, ssq_out) need the AFFINE_NORM mode", tag);
+  SAB_CHECK(!P.out_scaled || P.colscale, "%s: out_scaled needs colscale", tag);
+  SAB_CHECK(!(P.gate || P.out_scaled) || P.gate_div > 0, "%s: gate_div=%d must be > 0", tag, P.gate_div);
+  // the fused-norm consumer (rstd * acc + ibias) exists in the SwiGLU and plain QKV epilogues only
+  SAB_CHECK(!(P.ssq_in && affine), "%s: the fused-norm consumer (ssq_in) is not applied in the affine modes", tag);
+  SAB_CHECK(!(P.ssq_in && P.xa_kv), "%s: the fused-norm consumer (ssq_in) is not applied with fused cross-attention (xa_kv)", tag);
+  SAB_CHECK(!P.ssq_in || (P.ssq_n > 0 && P.ibias), "%s: ssq_in needs ssq_n > 0 and ibias", tag);
+  SAB_CHECK(!P.ibias || P.ibias_div > 0, "%s: ibias_div=%d must be > 0", tag, P.ibias_div);
+  if (mode == EPI_QKV) {
+    SAB_CHECK(!P.use_rope || (P.rope && P.rope_T > 0), "%s: use_rope needs rope and rope_T > 0", tag);
+    SAB_CHECK(P.rope_T > 0, "%s: rope_T=%d must be > 0 (RoPE positions are row %% rope_T)", tag, P.rope_T);
+  }
+  if (P.xa_kv) {
+    SAB_CHECK(mode == EPI_QKV, "%s: fused cross-attention (xa_kv) needs the QKV mode", tag);
+    SAB_CHECK(P.xa_Tk >= 1 && P.xa_Tk <= XA_MAX_TK, "%s: xa_Tk=%d outside 1..%d", tag, P.xa_Tk, XA_MAX_TK);
+    SAB_CHECK(P.xa_T >= 1, "%s: xa_T=%d must be >= 1", tag, P.xa_T);
+    SAB_CHECK(P.qnorm_w && P.n_q_end >= P.N, "%s: fused cross-attention needs q-norm weights on every column", tag);
+  }
+  if (b2b) {
+    SAB_CHECK(BN == P.N, "%s: back-to-back tiles need BN == N (BN=%d, N=%d)", tag, BN, P.N);
+    SAB_CHECK(cg == 1, "%s: back-to-back tiles need cg == 1 (cg=%d)", tag, cg);
+    SAB_CHECK(mode == EPI_AFFINE, "%s: back-to-back tiles need the affine mode (mode=%d)", tag, mode);
+    SAB_CHECK(!P.gate, "%s: back-to-back tiles apply no gate", tag);
+    SAB_CHECK(P.b2b_bias && P.b2b_alpha, "%s: back-to-back tiles need b2b_bias and b2b_alpha", tag);
+  }
+  SAB_CHECK(cg == 1 || cg == 2, "%s: cg=%d must be 1 or 2", tag, cg);
+  SAB_CHECK(grid > 0 && grid % cg == 0, "%s: grid of %d CTAs is not a multiple of cg=%d", tag, grid, cg);
+  SAB_CHECK(P.group_m >= 1 && (P.reverse_m == 0 || P.reverse_m == 1), "%s: group_m=%d / reverse_m=%d out of range", tag,
+            P.group_m, P.reverse_m);
+  int kb[2] = {0, 0};
+  for (int l = 0; l < 2; ++l) {
+    SAB_CHECK(P.n_runs[l] >= 0 && P.n_runs[l] <= GEMM_MAX_RUNS, "%s: %d K runs (at most %d)", tag, P.n_runs[l],
+              GEMM_MAX_RUNS);
+    for (int r = 0; r < P.n_runs[l]; ++r) {
+      SAB_CHECK(P.runs[l][r].nkb > 0, "%s: K run with %d k-blocks", tag, P.runs[l][r].nkb);
+      kb[l] += P.runs[l][r].nkb;
+    }
+  }
+  SAB_CHECK(kb[0] > 0, "%s: empty K run list", tag);
+  if (P.n_period > 0) {
+    SAB_CHECK(kb[1] == kb[0], "%s: run lists differ in K (%d vs %d k-blocks)", tag, kb[0], kb[1]);
+    SAB_CHECK(P.n_switch % BN == 0 && P.n_period % BN == 0, "%s: BN=%d does not divide the tap switch %d/%d", tag, BN,
+              P.n_switch, P.n_period);
+  }
+  SAB_CHECK(gemm_launcher(BN, BK, mode, cg, b2b) != nullptr,
+            "%s: no GEMM instantiation for BN=%d BK=%d mode=%d cg=%d b2b=%d", tag, BN, BK, mode, cg, (int)b2b);
+}
+
+static void launch_gemm(const GemmOp& op, cudaStream_t st) {
+  check_gemm(op.tag, op.BN, op.BK, op.mode, op.cg, op.b2b, op.grid, op.P);
+  gemm_launcher(op.BN, op.BK, op.mode, op.cg, op.b2b)(op, st);
 }
 
 // A operand view
@@ -149,7 +217,16 @@ struct RunList {
   }
 };
 
-static int g_force_cg = 0;   // SAB_FORCE_CG=1|2 overrides the CTA-group choice (A/B measurements)
+static int g_force_cg = 0;   // SAB_FORCE_CG=1|2 overrides the automatic CTA-group choice (A/B measurements)
+
+// cg = 0: the automatic choice — 2-CTA clusters (256 x BN tiles, B tile multicast to both CTAs) for the big
+// tensor-bound GEMMs, unless SAB_FORCE_CG overrides it.  An explicit cg always wins.
+static int pick_cg(const AView& A, int BN, int BK, int cg) {
+  if (cg != 0) return cg;
+  if (BN != 256 || BK != 64) return 1;
+  if (g_force_cg) return g_force_cg;
+  return (A.rows * A.items >= 1024 && A.rows >= 200) ? 2 : 1;
+}
 
 static GemmOp make_gemm(const char* tag, const AView& A, const bf16* B, int N, int BN, int BK, int mode,
                         const RunList& runs, int cg = 0) {
@@ -157,9 +234,7 @@ static GemmOp make_gemm(const char* tag, const AView& A, const bf16* B, int N, i
   memset(&op.P, 0, sizeof(op.P));
   op.tag = tag;
   op.BN = BN; op.BK = BK; op.mode = mode;
-  // 2-CTA clusters (256 x BN tiles, B tile multicast to both CTAs) for the big tensor-bound GEMMs
-  if (cg == 0) cg = (BN == 256 && BK == 64 && A.rows * A.items >= 1024 && A.rows >= 200) ? 2 : 1;
-  if (g_force_cg && BN == 256 && BK == 64) cg = g_force_cg;
+  cg = pick_cg(A, BN, BK, cg);
   op.cg = cg;
   const int ktot = runs.total_kb(0) * BK;
   if (runs.period > 0) SAB_CHECK(runs.total_kb(1) * BK == ktot, "%s: run lists differ in K", tag);
@@ -1301,8 +1376,14 @@ int sab_create(const sab_config* cfg, int device, sab_engine** out) {
   SAB_CUDA(cudaGetDeviceProperties(&prop, device));
   SAB_CHECK(prop.major == 9 && prop.minor == 0, "device %d is sm_%d%d; this library is built for sm_90a only", device,
             prop.major, prop.minor);
-  if (const char* f = getenv("SAB_FORCE_CG")) g_force_cg = atoi(f);
-  if (const char* f = getenv("SAB_ATTN_POLY")) g_attn_poly = atoi(f);
+  // the A/B switches are re-read by every engine: an unset variable restores the default for engines created later
+  {
+    const char* f = getenv("SAB_FORCE_CG");
+    g_force_cg = f ? atoi(f) : 0;
+    SAB_CHECK(g_force_cg >= 0 && g_force_cg <= 2, "SAB_FORCE_CG=%s: expected 1 or 2", f);
+    f = getenv("SAB_ATTN_POLY");
+    g_attn_poly = f ? atoi(f) : 2;
+  }
   g_serpentine = getenv("SAB_NO_SERPENTINE") == nullptr;
   SAB_CHECK(cfg->dim % 128 == 0 && cfg->dim / cfg->n_heads == 128, "dim must be n_heads*128");
   SAB_CHECK(cfg->ffn_hidden % 64 == 0, "ffn_hidden must be a multiple of 64");
@@ -1788,6 +1869,74 @@ int sab_test_gemm(int M, int N, int K, const void* a_bf16, const void* b_bf16, f
   rl.add(0, 0, 0, K / bk);
   GemmOp op = make_gemm("test", flat_view((const bf16*)a_bf16, M, K), (const bf16*)b_bf16, N, bn, bk, EPI_AFFINE, rl, cg);
   op.P.out_f32 = c; op.P.out_f32_ld = N;
+  launch_gemm(op, (cudaStream_t)stream);
+  SAB_API_END
+}
+
+// the descriptor's run lists and epilogue fields, copied into the kernel parameters
+static void desc_to_params(const sab_test_gemm_desc& d, GemmParams& P) {
+  P.N = d.n;
+  for (int l = 0; l < 2; ++l) {
+    P.n_runs[l] = d.n_runs[l];
+    for (int r = 0; r < GEMM_MAX_RUNS; ++r) P.runs[l][r] = KRun{d.runs[l][r].row_shift, d.runs[l][r].a_col, d.runs[l][r].nkb};
+  }
+  P.n_period = d.n_period; P.n_switch = d.n_switch;
+  P.bias = d.bias; P.bias_mod = d.bias_mod;
+  P.gate = d.gate; P.gate_ld = d.gate_ld; P.gate_div = d.gate_div;
+  P.alpha = d.alpha; P.relu = d.relu;
+  P.res = d.res; P.res_ld = d.res_ld;
+  P.out_f32 = d.out_f32; P.out_f32_ld = d.out_f32_ld;
+  P.out_bf16 = (bf16*)d.out_bf16; P.out_bf16_ld = d.out_bf16_ld;
+  P.out_act = (bf16*)d.out_act; P.out_act_ld = d.out_act_ld; P.snake_alpha = d.snake_alpha;
+  P.colscale = d.colscale; P.colscale_ld = d.colscale_ld;
+  P.out_scaled = (bf16*)d.out_scaled; P.out_scaled_ld = d.out_scaled_ld;
+  P.ssq_out = d.ssq_out; P.ssq_ld = d.ssq_ld;
+  P.ssq_in = d.ssq_in; P.ssq_n = d.ssq_n; P.ssq_inv_dim = d.ssq_inv_dim;
+  P.ibias = d.ibias; P.ibias_ld = d.ibias_ld; P.ibias_div = d.ibias_div;
+  P.b2b_bias = d.b2b_bias; P.b2b_alpha = d.b2b_alpha;
+  P.qnorm_w = d.qnorm_w; P.knorm_w = d.knorm_w;
+  P.n_q_end = d.n_q_end; P.n_k_end = d.n_k_end; P.qkv_period = d.qkv_period; P.norm_w_stride = d.norm_w_stride;
+  P.rope = (const float2*)d.rope; P.rope_T = d.rope_T; P.use_rope = d.use_rope; P.eps = d.eps;
+  P.xa_kv = (const bf16*)d.xa_kv; P.xa_kv_ld = d.xa_kv_ld; P.xa_v_col0 = d.xa_v_col0; P.xa_Tk = d.xa_Tk; P.xa_T = d.xa_T;
+  P.xa_mask = d.xa_mask; P.xa_scale_log2 = d.xa_scale_log2;
+}
+
+int sab_test_gemm_ex(const sab_test_gemm_desc* d, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(d != nullptr, "null descriptor");
+  SAB_CHECK(d->struct_bytes == (int32_t)sizeof(sab_test_gemm_desc),
+            "sab_test_gemm_desc.struct_bytes=%d but the library's descriptor has %d bytes (header and binding differ)",
+            d->struct_bytes, (int)sizeof(sab_test_gemm_desc));
+  SAB_CHECK(d->a && d->b && (!d->b2b || d->w1), "null A / B / w1 operand");
+  SAB_CHECK(d->a_cols > 0 && d->a_rows > 0 && d->a_items > 0, "empty A view");
+  SAB_CHECK(d->grid_ctas >= 0 && d->group_m >= 0, "grid_ctas / group_m must be >= 0 (0: engine default)");
+  for (int l = 0; l < 2; ++l)
+    SAB_CHECK(d->n_runs[l] >= 0 && d->n_runs[l] <= GEMM_MAX_RUNS, "%d K runs (at most %d)", d->n_runs[l], GEMM_MAX_RUNS);
+  const AView A{(const bf16*)d->a, d->a_cols, d->a_rows, d->a_items, d->a_row_pitch ? d->a_row_pitch : d->a_cols,
+                d->a_item_pitch};
+  RunList rl;
+  for (int l = 0; l < 2; ++l)
+    for (int r = 0; r < d->n_runs[l]; ++r) rl.add(l, d->runs[l][r].row_shift, d->runs[l][r].a_col, d->runs[l][r].nkb);
+  rl.period = d->n_period; rl.sw = d->n_switch;
+  // every rule the engine's own launches obey, before any CUDA call
+  const int cg = pick_cg(A, d->bn, d->bk, d->cg);
+  {
+    GemmParams pre;
+    memset(&pre, 0, sizeof(pre));
+    desc_to_params(*d, pre);
+    pre.group_m = d->group_m ? d->group_m : 1;
+    pre.reverse_m = d->reverse_m;
+    check_gemm("sab_test_gemm_ex", d->bn, d->bk, d->mode, cg, d->b2b != 0, d->grid_ctas ? d->grid_ctas : cg, pre);
+  }
+  GemmOp op = make_gemm("sab_test_gemm_ex", A, (const bf16*)d->b, d->n, d->bn, d->bk, d->mode, rl, cg);
+  desc_to_params(*d, op.P);   // (the tiling fields stay the planner's)
+  if (d->group_m) op.P.group_m = d->group_m;
+  op.P.reverse_m = d->reverse_m;
+  if (d->grid_ctas) op.grid = d->grid_ctas;
+  if (d->b2b) {
+    op.b2b = true;
+    op.tmW = make_tmap_2d(d->w1, d->n, d->n, d->n, d->bk, d->bn);
+  }
   launch_gemm(op, (cudaStream_t)stream);
   SAB_API_END
 }

@@ -75,7 +75,8 @@ struct GemmParams {
   //     =  rstd[row] * ((h * w*(1+scale)) @ W^T)  +  shift @ W^T
   //  producer (affine epilogue): out_scaled = bf16(v * colscale[row / gate_div][n]) is the consumer's A operand and
   //    ssq_out[row, 2*n_tile + parity] = sum of v^2 over the tile's even (parity 0) or odd 32-column chunks (no atomics);
-  //  consumer (every mode): acc' = rstd[row] * acc + ibias[row / ibias_div][n] before anything else,
+  //  consumer (SwiGLU and QKV without fused cross-attention; the host rejects ssq_in elsewhere):
+  //    acc' = rstd[row] * acc + ibias[row / ibias_div][n] before anything else,
   //    rstd[row] = rsqrt(sum_j ssq_in[row, j] * ssq_inv_dim + eps),  ibias = shift @ W^T (one small GEMM per evaluation)
   const float* colscale; long long colscale_ld;      // item = row / gate_div (as for the adaLN gate)
   __nv_bfloat16* out_scaled; long long out_scaled_ld;
