@@ -198,8 +198,20 @@ typedef struct sab_test_gemm_desc {
   const void* rope; int32_t rope_T, use_rope; float eps;   /* rope: [rope_T, 64] (cos, sin) float pairs */
   const void* xa_kv; int64_t xa_kv_ld; int32_t xa_v_col0, xa_Tk, xa_T;
   const uint8_t* xa_mask; float xa_scale_log2;
+  /* per-clip B: item i multiplies rows (i / b_clip_div) * b_clip_rows + [0, n) of b, which then has
+   * ceil(a_items / b_clip_div) * b_clip_rows rows of b_cols visible columns at pitch b_ld (0: the run list's K) */
+  int32_t b_clip_rows, b_clip_div;
+  int64_t b_cols, b_ld;
+  /* fused cross-attention writes its probabilities [rows, xa_Tk * heads] (bf16, column j * heads + h) here instead of O */
+  void* xa_p; int64_t xa_p_ld;
 } sab_test_gemm_desc;
 int sab_test_gemm_ex(const sab_test_gemm_desc* d, void* stream);
+/* The cross-attention fold (sam_audio_b200/csrc/xattn_fold.cuh) for `layers` layers:
+ *   ut[l * ut_layer_stride + (b * d + n) * ldu + j * heads + h] = bf16(sum_c Wo_l[n, h*128 + c] * V_l[b*L + j, h*128 + c])
+ * with d = heads * 128, Wo_l = wo_table[l] (a DEVICE array of layers pointers to [d, d] bf16) and
+ * V_l[r, c] = kv[r * kv_ld + l * kv_layer_cols + v_col0 + c] (bf16, clips * L rows); columns [heads * L, ldu) are 0. */
+int sab_test_xattn_fold(int layers, int clips, int L, int heads, const void* wo_table, const void* kv, int64_t kv_ld,
+                        int64_t kv_layer_cols, int v_col0, void* ut, int ldu, int64_t ut_layer_stride, void* stream);
 /* O = softmax(Q K^T / sqrt(128) + mask) V through the attention kernel; all [items*T, heads*128] bf16. */
 int sab_test_attention(int items, int heads, int Tq, int Tk, const void* q, const void* k, const void* v,
                        const uint8_t* key_mask, void* o, void* stream);

@@ -68,6 +68,8 @@ class SabTestGemmDesc(ctypes.Structure):
         ("rope", _vp), ("rope_T", _i32), ("use_rope", _i32), ("eps", _f32),
         ("xa_kv", _vp), ("xa_kv_ld", _i64), ("xa_v_col0", _i32), ("xa_Tk", _i32), ("xa_T", _i32),
         ("xa_mask", _vp), ("xa_scale_log2", _f32),
+        ("b_clip_rows", _i32), ("b_clip_div", _i32), ("b_cols", _i64), ("b_ld", _i64),
+        ("xa_p", _vp), ("xa_p_ld", _i64),
     ]
 
     def __init__(self, **kw):
@@ -81,7 +83,7 @@ class SabTestGemmDesc(ctypes.Structure):
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
-    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_attention", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -118,6 +120,7 @@ def lib() -> ctypes.CDLL:
         L.sab_profile_report.argtypes = [vp, ctypes.c_char_p, i64, vp]
         L.sab_test_gemm.argtypes = [i32, i32, i32, vp, vp, vp, i32, i32, i32, vp]
         L.sab_test_gemm_ex.argtypes = [ctypes.POINTER(SabTestGemmDesc), vp]
+        L.sab_test_xattn_fold.argtypes = [i32, i32, i32, i32, vp, vp, i64, i64, i32, vp, i32, i64, vp]
         L.sab_test_attention.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
         L.sab_test_attention_tc2.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp]
         L.sab_preprocess_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]

@@ -18,6 +18,7 @@
 #include "elementwise.cuh"
 #include "codec_kernels.cuh"
 #include "vision_kernels.cuh"
+#include "xattn_fold.cuh"
 
 using namespace sab;
 typedef __nv_bfloat16 bf16;
@@ -67,9 +68,9 @@ struct DeviceGuard {
 // =====================================================================================================
 // GEMM dispatch
 // =====================================================================================================
-template <int BN, int BK, int MODE, int CG, bool B2B = false>
+template <int BN, int BK, int MODE, int CG, bool B2B = false, bool XAP = false>
 static void launch_gemm_inst(const GemmOp& op, cudaStream_t st) {
-  auto kern = gemm_tc_kernel<BN, BK, MODE, CG, B2B>;
+  auto kern = gemm_tc_kernel<BN, BK, MODE, CG, B2B, XAP>;
   constexpr int smem = GemmSmem<BN, BK, CG, B2B>::kTotal;
   ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
   if (CG == 1) {
@@ -92,9 +93,16 @@ static void launch_gemm_inst(const GemmOp& op, cudaStream_t st) {
   SAB_CUDA(cudaGetLastError());
 }
 
-// the instantiation table: the launcher of (BN, BK, mode, cg, b2b), or nullptr if that combination is not built
+// the instantiation table: the launcher of (BN, BK, mode, cg, b2b, xap = cross-attention probabilities out), or nullptr
+// if that combination is not built
 typedef void (*GemmLauncher)(const GemmOp&, cudaStream_t);
-static GemmLauncher gemm_launcher(int BN, int BK, int mode, int cg, bool b2b) {
+static GemmLauncher gemm_launcher(int BN, int BK, int mode, int cg, bool b2b, bool xap) {
+  if (xap) {
+    if (BN != 256 || BK != 64 || mode != EPI_QKV || b2b) return nullptr;
+    if (cg == 2) return launch_gemm_inst<256, 64, EPI_QKV, 2, false, true>;
+    if (cg == 1) return launch_gemm_inst<256, 64, EPI_QKV, 1, false, true>;
+    return nullptr;
+  }
   if (b2b) {
     if (mode != EPI_AFFINE || cg != 1) return nullptr;
     if (BN == 64 && BK == 64) return launch_gemm_inst<64, 64, EPI_AFFINE, 1, true>;
@@ -132,7 +140,16 @@ static void check_gemm(const char* tag, int BN, int BK, int mode, int cg, bool b
   SAB_CHECK(P.N > 0 && P.N % 32 == 0, "%s: N=%d must be a positive multiple of 32", tag, P.N);
   SAB_CHECK(mode != EPI_QKV || P.N % 128 == 0, "%s: QKV mode needs whole 128-column heads (N=%d)", tag, P.N);
   SAB_CHECK(mode != EPI_SWIGLU || P.N % 64 == 0, "%s: SwiGLU mode needs whole [32 gate | 32 up] pairs (N=%d)", tag, P.N);
-  SAB_CHECK(affine || P.out_bf16, "%s: SwiGLU / QKV modes write out_bf16, which is not set", tag);
+  SAB_CHECK(!P.xa_p || P.xa_kv, "%s: xa_p (cross-attention probabilities) needs fused cross-attention (xa_kv)", tag);
+  SAB_CHECK(affine || P.out_bf16 || P.xa_p, "%s: SwiGLU / QKV modes write out_bf16, which is not set", tag);
+  SAB_CHECK(P.b_clip_rows >= 0, "%s: b_clip_rows=%d must be >= 0", tag, P.b_clip_rows);
+  if (P.b_clip_rows > 0) {
+    SAB_CHECK(P.b_clip_div >= 1, "%s: b_clip_div=%d must be >= 1 with a per-clip B (b_clip_rows=%d)", tag, P.b_clip_div,
+              P.b_clip_rows);
+    SAB_CHECK(P.b_clip_rows >= P.N, "%s: b_clip_rows=%d must be >= N=%d (a clip's B holds all N rows)", tag,
+              P.b_clip_rows, P.N);
+    SAB_CHECK(!b2b, "%s: back-to-back tiles have no per-clip B", tag);
+  }
   SAB_CHECK(!P.out_act || P.snake_alpha, "%s: out_act needs snake_alpha", tag);
   SAB_CHECK(mode == EPI_AFFINE_NORM || (!P.out_scaled && !P.ssq_out),
             "%s: the fused-norm producer outputs (out_scaled, ssq_out) need the AFFINE_NORM mode", tag);
@@ -152,6 +169,8 @@ static void check_gemm(const char* tag, int BN, int BK, int mode, int cg, bool b
     SAB_CHECK(P.xa_Tk >= 1 && P.xa_Tk <= XA_MAX_TK, "%s: xa_Tk=%d outside 1..%d", tag, P.xa_Tk, XA_MAX_TK);
     SAB_CHECK(P.xa_T >= 1, "%s: xa_T=%d must be >= 1", tag, P.xa_T);
     SAB_CHECK(P.qnorm_w && P.n_q_end >= P.N, "%s: fused cross-attention needs q-norm weights on every column", tag);
+    SAB_CHECK(!P.xa_p || P.xa_p_ld >= (long long)(P.N / 128) * P.xa_Tk,
+              "%s: xa_p_ld=%lld is below heads * xa_Tk = %d", tag, P.xa_p_ld, (P.N / 128) * P.xa_Tk);
   }
   if (b2b) {
     SAB_CHECK(BN == P.N, "%s: back-to-back tiles need BN == N (BN=%d, N=%d)", tag, BN, P.N);
@@ -179,13 +198,14 @@ static void check_gemm(const char* tag, int BN, int BK, int mode, int cg, bool b
     SAB_CHECK(P.n_switch % BN == 0 && P.n_period % BN == 0, "%s: BN=%d does not divide the tap switch %d/%d", tag, BN,
               P.n_switch, P.n_period);
   }
-  SAB_CHECK(gemm_launcher(BN, BK, mode, cg, b2b) != nullptr,
-            "%s: no GEMM instantiation for BN=%d BK=%d mode=%d cg=%d b2b=%d", tag, BN, BK, mode, cg, (int)b2b);
+  SAB_CHECK(gemm_launcher(BN, BK, mode, cg, b2b, P.xa_p != nullptr) != nullptr,
+            "%s: no GEMM instantiation for BN=%d BK=%d mode=%d cg=%d b2b=%d%s", tag, BN, BK, mode, cg, (int)b2b,
+            P.xa_p ? " with xa_p" : "");
 }
 
 static void launch_gemm(const GemmOp& op, cudaStream_t st) {
   check_gemm(op.tag, op.BN, op.BK, op.mode, op.cg, op.b2b, op.grid, op.P);
-  gemm_launcher(op.BN, op.BK, op.mode, op.cg, op.b2b)(op, st);
+  gemm_launcher(op.BN, op.BK, op.mode, op.cg, op.b2b, op.P.xa_p != nullptr)(op, st);
 }
 
 // A operand view
@@ -278,6 +298,20 @@ static GemmOp make_linear(const char* tag, const bf16* A, int64_t M, int K, cons
   RunList rl;
   rl.add(0, 0, 0, K / 64);
   return make_gemm(tag, flat_view(A, M, K, lda), B, N, BN, 64, mode, rl);
+}
+// Per-clip B: item i of the GEMM multiplies rows (i / clip_div) * clip_rows + [0, N) of B [n_clips * clip_rows, b_cols]
+// (row pitch b_ld elements; TMA zero-fills the k-block columns past b_cols).  FLOPs count K = b_cols and the bytes
+// count each clip's B once.
+static void set_per_clip_b(GemmOp& op, const bf16* B, int64_t b_cols, int64_t b_ld, int clip_rows, int clip_div) {
+  SAB_CHECK(clip_rows > 0 && clip_div > 0, "%s: per-clip B needs clip_rows > 0 and clip_div > 0", op.tag);
+  int ktot = 0;
+  for (int r = 0; r < op.P.n_runs[0]; ++r) ktot += op.P.runs[0][r].nkb * op.BK;
+  const int64_t n_clips = (op.P.n_items + clip_div - 1) / clip_div;
+  op.tmB = make_tmap_2d(B, b_cols, n_clips * clip_rows, b_ld, op.BK, op.BN / op.cg);
+  op.P.b_clip_rows = clip_rows;
+  op.P.b_clip_div = clip_div;
+  op.in_bytes += (double)op.P.N * ((double)n_clips * (double)b_cols - (double)ktot) * 2.0;
+  op.flops = 2.0 * op.rows * (double)op.P.N * (double)b_cols;
 }
 
 // =====================================================================================================
@@ -674,6 +708,13 @@ struct DitPlan {
   CUtensorMap tm_att_q, tm_att_kv;   // fused-QKV buffer viewed as (3d cols, T rows, Bc items): box 64x128 / 64x256
   bool att_tc = false;               // wgmma self-attention usable (T <= 256)
   bool xa_fused = false;             // cross-attention folded into the cross.wq GEMM epilogue (L <= XA_MAX_TK)
+  // ... and cross.wo folded into the text values (xattn_fold.cuh): cross.wq writes the probabilities xa_p [M, ldu],
+  // cross.wo is a K = heads * L GEMM against the clip's Ut[l] [B * d, ldu], computed once per evaluation
+  bool xa_fold = false;
+  int ldu = 0;
+  bf16 *xa_p = nullptr, *ut = nullptr;
+  const bf16** wo_c_tab = nullptr;   // [NL] device copy of the layers' cross wo pointers
+  double fold_flops = 0, fold_bytes = 0;
   double flops_per_eval = 0;
   // the whole ODE solve (2*n_steps evaluations for midpoint, ~5.9k launches at 24 layers) as one CUDA graph, captured on the second solve
   // of a plan (the first one runs eagerly and configures every kernel's attributes)
@@ -804,6 +845,16 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
   // ---- layers ----
   p.lay.resize(NL);
   p.xa_fused = (L <= XA_MAX_TK) && !getenv("SAB_NO_FUSED_XATTN");
+  p.xa_fold = p.xa_fused && !getenv("SAB_NO_XATTN_FOLD");
+  if (p.xa_fold) {
+    p.ldu = (c.n_heads * L + 7) / 8 * 8;   // Ut / P row pitch: 16-byte TMA strides
+    p.xa_p = w.alloc<bf16>(M * p.ldu);
+    p.ut = w.alloc<bf16>((int64_t)NL * B * d * p.ldu);
+    std::vector<const bf16*> tab(NL);
+    for (int l = 0; l < NL; ++l) tab[l] = e->layers[l].wo_c;
+    p.wo_c_tab = w.alloc<const bf16*>(NL);
+    SAB_CUDA(cudaMemcpy(p.wo_c_tab, tab.data(), NL * sizeof(const bf16*), cudaMemcpyHostToDevice));
+  }
   for (int l = 0; l < NL; ++l) {
     const LayerW& W = e->layers[l];
     LayerOps& o = p.lay[l];
@@ -832,8 +883,19 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
       o.q_c.P.xa_scale_log2 = (1.0f / sqrtf(128.f)) * 1.4426950408889634f;
       o.q_c.flops += 4.0 * Bc * c.n_heads * (double)T * L * 128;
     }
-
-    o.wo_c = make_linear("cross.wo", p.att, M, d, W.wo_c, d, 256, EPI_AFFINE);
+    if (p.xa_fold) {    // ... its probabilities only: cross.wo multiplies them with the clip's folded values Ut[l]
+      o.q_c.P.out_bf16 = nullptr; o.q_c.P.out_bf16_ld = 0;
+      o.q_c.P.xa_p = p.xa_p; o.q_c.P.xa_p_ld = p.ldu;
+      o.q_c.flops -= 2.0 * Bc * c.n_heads * (double)T * L * 128;   // no P V
+      RunList rl;
+      rl.add(0, 0, 0, (c.n_heads * L + 63) / 64);
+      const bf16* ut_l = p.ut + (int64_t)l * B * d * p.ldu;
+      o.wo_c = make_gemm("cross.wo", AView{p.xa_p, (int64_t)c.n_heads * L, T, Bc, p.ldu, (int64_t)T * p.ldu}, ut_l, d,
+                         256, 64, EPI_AFFINE, rl);
+      set_per_clip_b(o.wo_c, ut_l, (int64_t)c.n_heads * L, p.ldu, d, cand);
+    } else {
+      o.wo_c = make_linear("cross.wo", p.att, M, d, W.wo_c, d, 256, EPI_AFFINE);
+    }
     o.wo_c.P.res = p.h; o.wo_c.P.res_ld = d; o.wo_c.P.out_f32 = p.h; o.wo_c.P.out_f32_ld = d;
     norm_producer(o.wo_c, 2 * l + 1);
     o.w13 = make_linear("ffn.w13", p.xn, M, d, W.w13, 2 * hid, 256, EPI_SWIGLU);
@@ -863,6 +925,11 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
   for (auto& o : p.lay)
     f += o.qkv.flops + o.wo.flops + o.q_c.flops + o.wo_c.flops + o.w13.flops + o.w2.flops +
          4.0 * Bc * (double)T * T * d + 4.0 * Bc * (double)T * L * d;
+  if (p.xa_fold) {   // Wo of every layer read once, V read once, Ut written once
+    p.fold_flops = 2.0 * NL * (double)B * d * c.n_heads * L * 128;
+    p.fold_bytes = (double)NL * ((double)d * d * 2.0 + (double)ML * d * 2.0 + (double)B * d * p.ldu * 2.0);
+    f += p.fold_flops;
+  }
   p.flops_per_eval = f;
   e->dit = std::move(P);
 }
@@ -939,6 +1006,26 @@ static void launch_attention_tc2(const CUtensorMap& tq, const CUtensorMap& tk, c
     default: throw Error(fmt("SAB_ATTN_POLY=%d not built (0, 2, 3, 4)", g_attn_poly));
   }
 #undef SAB_AT2
+}
+
+// xattn_fold.cuh: every layer's Ut in one launch.  A CTA sweeps the clips in chunks whose Ut rows it holds in shared
+// memory; chunks are sized to about 96 KB so that two CTAs share an SM.
+constexpr int XF_MAX_SMEM = 200 * 1024;
+static void launch_xattn_fold(XaFoldParams fp, int layers, cudaStream_t st) {
+  SAB_CHECK(fp.L >= 1 && fp.L <= XA_MAX_TK, "cross.fold: L=%d outside 1..%d", fp.L, XA_MAX_TK);
+  SAB_CHECK(fp.heads * 128 == fp.d && fp.d % XF_ROWS == 0, "cross.fold: d=%d must be heads x 128 (heads=%d)", fp.d, fp.heads);
+  SAB_CHECK(fp.ldu % 8 == 0 && fp.ldu >= fp.heads * fp.L, "cross.fold: ldu=%d must be a multiple of 8 and >= heads*L=%d",
+            fp.ldu, fp.heads * fp.L);
+  SAB_CHECK(fp.clips >= 1 && layers >= 1, "cross.fold: empty launch");
+  const int clip_bytes = XF_ROWS * fp.ldu * 2;
+  const int max_chunk = std::max(1, 96 * 1024 / clip_bytes);
+  const int n_chunks = (fp.clips + max_chunk - 1) / max_chunk;
+  fp.chunk = (fp.clips + n_chunks - 1) / n_chunks;
+  const int smem = fp.chunk * clip_bytes;
+  SAB_CHECK(smem <= XF_MAX_SMEM, "cross.fold: %d bytes of shared memory per clip chunk", smem);
+  ensure_dynamic_smem(reinterpret_cast<const void*>(xattn_fold_kernel), XF_MAX_SMEM);
+  xattn_fold_kernel<<<dim3(fp.d / XF_ROWS, layers), XF_THREADS, smem, st>>>(fp);
+  SAB_CUDA(cudaGetLastError());
 }
 
 static void gemm(sab_engine* e, const GemmOp& op, cudaStream_t st) {
@@ -1026,6 +1113,15 @@ static void dit_eval(sab_engine* e, const float* time_dev, const FinalSpec& fs, 
   }
   SAB_CUDA(cudaGetLastError());
   gemm(e, p.g_kvc_all, st);
+  if (p.xa_fold) {
+    XaFoldParams fp{};
+    fp.wo = p.wo_c_tab;
+    fp.kv = p.kvc; fp.kv_ld = 2LL * d * NL; fp.kv_layer_cols = 2LL * d; fp.v_col0 = d;
+    fp.ut = p.ut; fp.ut_layer_stride = (long long)p.B * d * p.ldu; fp.ldu = p.ldu;
+    fp.d = d; fp.heads = H; fp.L = L; fp.clips = p.B;
+    mark(e, st, "cross.fold", p.fold_flops, p.fold_bytes);
+    launch_xattn_fold(fp, NL, st);
+  }
   int dir = 1;   // x_embedder.conv2 (the producer of h) walked the rows forwards
   for (int l = 0; l < NL; ++l) {
     const LayerW& W = e->layers[l];
@@ -1899,6 +1995,8 @@ static void desc_to_params(const sab_test_gemm_desc& d, GemmParams& P) {
   P.rope = (const float2*)d.rope; P.rope_T = d.rope_T; P.use_rope = d.use_rope; P.eps = d.eps;
   P.xa_kv = (const bf16*)d.xa_kv; P.xa_kv_ld = d.xa_kv_ld; P.xa_v_col0 = d.xa_v_col0; P.xa_Tk = d.xa_Tk; P.xa_T = d.xa_T;
   P.xa_mask = d.xa_mask; P.xa_scale_log2 = d.xa_scale_log2;
+  P.xa_p = (bf16*)d.xa_p; P.xa_p_ld = d.xa_p_ld;
+  P.b_clip_rows = d.b_clip_rows; P.b_clip_div = d.b_clip_div;
 }
 
 int sab_test_gemm_ex(const sab_test_gemm_desc* d, void* stream) {
@@ -1933,11 +2031,31 @@ int sab_test_gemm_ex(const sab_test_gemm_desc* d, void* stream) {
   if (d->group_m) op.P.group_m = d->group_m;
   op.P.reverse_m = d->reverse_m;
   if (d->grid_ctas) op.grid = d->grid_ctas;
+  if (d->b_clip_rows > 0) {
+    const int64_t ktot = (int64_t)rl.total_kb(0) * d->bk;
+    set_per_clip_b(op, (const bf16*)d->b, d->b_cols ? d->b_cols : ktot, d->b_ld ? d->b_ld : ktot, d->b_clip_rows,
+                   d->b_clip_div);
+  }
   if (d->b2b) {
     op.b2b = true;
     op.tmW = make_tmap_2d(d->w1, d->n, d->n, d->n, d->bk, d->bn);
   }
   launch_gemm(op, (cudaStream_t)stream);
+  SAB_API_END
+}
+
+int sab_test_xattn_fold(int layers, int clips, int L, int heads, const void* wo_table, const void* kv, int64_t kv_ld,
+                        int64_t kv_layer_cols, int v_col0, void* ut, int ldu, int64_t ut_layer_stride, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(wo_table && kv && ut, "null operand");
+  SAB_CHECK(ut_layer_stride >= (int64_t)clips * heads * 128 * ldu, "ut_layer_stride=%lld is below clips * d * ldu",
+            (long long)ut_layer_stride);
+  XaFoldParams fp{};
+  fp.wo = (const bf16* const*)wo_table;
+  fp.kv = (const bf16*)kv; fp.kv_ld = kv_ld; fp.kv_layer_cols = kv_layer_cols; fp.v_col0 = v_col0;
+  fp.ut = (bf16*)ut; fp.ut_layer_stride = ut_layer_stride; fp.ldu = ldu;
+  fp.d = heads * 128; fp.heads = heads; fp.L = L; fp.clips = clips;
+  launch_xattn_fold(fp, layers, (cudaStream_t)stream);
   SAB_API_END
 }
 

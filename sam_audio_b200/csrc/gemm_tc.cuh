@@ -27,7 +27,9 @@
 //      EPI_AFFINE : v = (acc + bias[n]) * gate[row/gate_div, n] * alpha + res[row, n]
 //                   -> fp32 and/or bf16 and/or Snake(v) bf16   (DiT residual/gate, ODE axpy, codec convs)
 //      EPI_SWIGLU : silu(gate_cols) * up_cols -> bf16          (w1|w3 interleaved in 32-col chunks)
-//      EPI_QKV    : per-head RMSNorm (q,k) + RoPE on adjacent pairs -> bf16   (heads are 128 contiguous cols)
+//      EPI_QKV    : per-head RMSNorm (q,k) + RoPE on adjacent pairs -> bf16   (heads are 128 contiguous cols);
+//                   or attention to a few text tokens -> O, or (XAP) -> the probabilities only
+//  * A per-clip B operand (b_clip_rows > 0) lets cross.wo multiply the probabilities with its clip's folded values.
 #pragma once
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -97,6 +99,12 @@ struct GemmParams {
   int xa_T;                 // query rows per K/V item (T x candidates: the candidates of a clip share its text K/V)
   const uint8_t* xa_mask;   // [items, Tk] or null
   float xa_scale_log2;
+  // ... or, with xa_p set (XAP instantiation), writes each row's normalised probabilities to xa_p[row, j * heads + head]
+  // (bf16; masked tokens exactly 0; token-major, so that a token's column does not depend on Tk) and no O: the output
+  // projection then runs as a per-clip GEMM over them (see b_clip_rows)
+  __nv_bfloat16* xa_p; long long xa_p_ld;
+  // per-clip B operand: item i multiplies rows (i / b_clip_div) * b_clip_rows + [0, N) of B (0: one B shared by all)
+  int b_clip_rows, b_clip_div;
 };
 constexpr int XA_MAX_TK = 8;
 
@@ -166,7 +174,9 @@ SAB_DEVICE void tile_coords(int tile, int n_tiles_m, int n_tiles_n, int group_m,
 
 SAB_DEVICE uint2 pack4_bf16(float4 v) { return make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w)); }
 
-template <int BN, int BK, int MODE, int CG, bool B2B = false>
+// XAP: the fused cross-attention writes probabilities (xa_p) instead of O (its own instantiation: the two epilogues
+// together do not fit the consumer's registers)
+template <int BN, int BK, int MODE, int CG, bool B2B = false, bool XAP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmW /*B2B: [BN, BN] second weight, box BK x BN*/,
@@ -182,6 +192,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   static_assert(BN != 256 || kStages >= 4, "256-wide tiles need at least 4 pipeline stages");
   static_assert(MODE != EPI_SWIGLU || BN % 64 == 0, "SwiGLU tiles hold whole [32 gate | 32 up] column pairs");
   static_assert(MODE != EPI_QKV || BN % 128 == 0, "QKV tiles hold whole 128-column heads");
+  static_assert(!XAP || MODE == EPI_QKV, "cross-attention probabilities come from the QKV epilogue");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -228,7 +239,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int item = mt / P.tiles_per_item;
         const int t0 = (mt % P.tiles_per_item) * (GEMM_BM * CG) + (int)cta_rank * GEMM_BM;
         const int n0 = nt * BN;
-        const int nb = n0 + (int)cta_rank * (BN / CG);   // this CTA's slice of the B tile
+        // this CTA's slice of the B tile (of the item's clip, for a per-clip B: both CTAs of a cluster share the item)
+        const int nb = n0 + (int)cta_rank * (BN / CG) + (P.b_clip_rows ? (item / P.b_clip_div) * P.b_clip_rows : 0);
         const int list = (P.n_period > 0 && (n0 % P.n_period) >= P.n_switch) ? 1 : 0;
         int kb_global = 0;
         for (int r = 0; r < P.n_runs[list]; ++r) {
@@ -587,7 +599,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const int nhp = P.qkv_period > 0 ? nh - rep * P.qkv_period : nh;
           const float* nw = (nhp < P.n_q_end) ? P.qnorm_w + rep * P.norm_w_stride
                                                : (nhp < P.n_k_end ? P.knorm_w + rep * P.norm_w_stride : nullptr);
-          if (P.xa_kv != nullptr) {
+          if (XAP || P.xa_kv != nullptr) {
             // ---- fused cross-attention to the row's text tokens (scores are linear in the un-normalised query).
             //      Scores in row form: both half-warps run the row's sum of squares, each the dot products of
             //      half of the tokens (j0 .. j0+3) ----
@@ -654,6 +666,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               den += pj;
             }
             const float inv = 1.f / den;
+            if constexpr (XAP) {   // probabilities only: lanes 0..15 hold rows 0..15 of the warp, Tk values each
+              if (lane < 16 && t_base + rr < P.rows_per_item) {
+                __nv_bfloat16* pp = P.xa_p + row_grow(rr) * P.xa_p_ld + (nh >> 7);
+#pragma unroll
+                for (int j = 0; j < XA_MAX_TK; ++j)
+                  if (j < P.xa_Tk) pp[j * (P.N >> 7)] = __float2bfloat16_rn(sc[j] * inv);
+              }
+            } else {
             // O = P V in fragment form, accumulated over the head's (no longer needed) accumulators: the
             // probabilities of the fragment rows fr and fr + 8 come from lanes fr and fr + 8
             float pf[2][XA_MAX_TK];
@@ -695,8 +715,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               for (int p = 0; p < 4; ++p)
                 if (4 * p < rl) *reinterpret_cast<uint2*>(o0 + p * st) = pack4_bf16(x[p]);
             }
+            }
             continue;
           }
+          if constexpr (XAP) continue;   // (never reached: XAP launches always carry xa_kv)
           float rs[4] = {1.f, 1.f, 1.f, 1.f};   // per-head RMSNorm rstd of each pass's row
           if (nw) {
             float ss = 0.f;   // of row rr, over the head's 128 columns in order
