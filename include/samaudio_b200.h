@@ -223,6 +223,17 @@ int sab_test_attention(int items, int heads, int Tq, int Tk, const void* q, cons
 int sab_test_attention_tc2(int items, int heads, int T, const void* q_bf16, const void* k_bf16, const void* v_bf16,
                            const uint8_t* key_mask, void* o_bf16, float shift_log2, int poly, void* stream);
 
+/* Same, through the wgmma streaming self-attention kernel (attention_stream_tc.cuh; any T, the engine uses it for
+ * T > 256): shift_log2 < 0 = exact online softmax, >= 0 = the bounded variant (q already scaled by log2(e)/sqrt(128),
+ * every |logit| <= shift_log2 <= 50 in the log2 domain; 0 stands for 50); poly as above. */
+int sab_test_attention_stream(int items, int heads, int T, const void* q_bf16, const void* k_bf16, const void* v_bf16,
+                              const uint8_t* key_mask, void* o_bf16, float shift_log2, int poly, void* stream);
+
+/* Time tiling of long clips in the codec (decoder != 0: sab_decode, else sab_encode) for a clip of T latent frames under
+ * the current workspace budget: halo_frames = latent frames of context an output frame needs on each side, derived from
+ * the codec's layer list; tile_frames = length of the tiles the clip is cut into, 0 when it runs whole. */
+int sab_codec_tiling(sab_engine* e, int decoder, int T, int* halo_frames, int* tile_frames);
+
 /* Visual prompting, frame pre-processing.  replaces: PerceptionEncoder.get_transform (vision_encoder.py:91-113) =
  * torchvision Resize((S, S), BICUBIC, antialias) on uint8 frames, x / 255, Normalize(0.5, 0.5).
  * frames [n_frames, 3, H, W] uint8 (device), workspace [n_frames, 3, H, S] fp32 (device), out [n_frames, 3, S, S] fp32.

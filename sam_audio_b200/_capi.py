@@ -83,7 +83,7 @@ class SabTestGemmDesc(ctypes.Structure):
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
-    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -123,6 +123,8 @@ def lib() -> ctypes.CDLL:
         L.sab_test_xattn_fold.argtypes = [i32, i32, i32, i32, vp, vp, i64, i64, i32, vp, i32, i64, vp]
         L.sab_test_attention.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
         L.sab_test_attention_tc2.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp]
+        L.sab_test_attention_stream.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp]
+        L.sab_codec_tiling.argtypes = [vp, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32)]
         L.sab_preprocess_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
         L.sab_test_aa_taps.argtypes = [i32, i32, i32, vp, vp, vp, vp]
         L.sab_test_solver_grid.argtypes = [i32, i32, i32, vp, vp]
@@ -252,6 +254,12 @@ class Engine:
         buf = ctypes.create_string_buffer(1 << 16)
         check(lib().sab_profile_report(self._h, buf, len(buf), stream_ptr()))
         return json.loads(buf.value.decode())
+
+    def codec_tiling(self, decoder: bool, T: int):
+        """(halo, tile length) in latent frames for a clip of T frames; tile length 0 = the clip runs whole."""
+        halo, tile = ctypes.c_int(), ctypes.c_int()
+        check(lib().sab_codec_tiling(self._h, 1 if decoder else 0, T, ctypes.byref(halo), ctypes.byref(tile)))
+        return halo.value, tile.value
 
     def workspace_bytes(self) -> int:
         return int(lib().sab_workspace_bytes(self._h))

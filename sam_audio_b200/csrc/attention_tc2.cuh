@@ -14,7 +14,7 @@
 // bound is small enough (<= 50) that p = 2^s needs neither scale nor shift.  kPoly of every 8 exponential pairs run
 // on the FMA pipe (Cody-Waite range reduction + degree-3 minimax polynomial, rel. error 7.5e-5, far below bf16's
 // 3.9e-3), the rest on the MUFU.
-// Longer sequences use the streaming kernel in attention.cuh.
+// Longer sequences use the wgmma streaming kernel in attention_stream_tc.cuh.
 #pragma once
 #include "common.cuh"
 #include "wgmma.cuh"

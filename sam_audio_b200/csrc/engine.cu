@@ -15,6 +15,7 @@
 #include "host_util.h"
 #include "attention.cuh"
 #include "attention_tc2.cuh"
+#include "attention_stream_tc.cuh"
 #include "elementwise.cuh"
 #include "codec_kernels.cuh"
 #include "vision_kernels.cuh"
@@ -706,7 +707,7 @@ struct DitPlan {
   GemmOp g_y13, g_y2, g_in, g_xe[2], g_out, g_cond, g_mem, g_vid, g_kvc_all;
   std::vector<LayerOps> lay;
   CUtensorMap tm_att_q, tm_att_kv;   // fused-QKV buffer viewed as (3d cols, T rows, Bc items): box 64x128 / 64x256
-  bool att_tc = false;               // wgmma self-attention usable (T <= 256)
+  bool att_tc = false;               // wgmma self-attention: attention_tc2 for T <= 256, attention_stream_tc above
   bool xa_fused = false;             // cross-attention folded into the cross.wq GEMM epilogue (L <= XA_MAX_TK)
   // ... and cross.wo folded into the text values (xattn_fold.cuh): cross.wq writes the probabilities xa_p [M, ldu],
   // cross.wo is a K = heads * L GEMM against the clip's Ut[l] [B * d, ldu], computed once per evaluation
@@ -913,10 +914,10 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
   p.g_kvc_all.P.qnorm_w = e->kn_c_all; p.g_kvc_all.P.knorm_w = e->kn_c_all;
   p.g_kvc_all.P.n_q_end = 0; p.g_kvc_all.P.n_k_end = d; p.g_kvc_all.P.qkv_period = 2 * d; p.g_kvc_all.P.norm_w_stride = 128;
   p.g_kvc_all.P.rope_T = L; p.g_kvc_all.P.use_rope = 0; p.g_kvc_all.P.eps = c.norm_eps;
-  p.att_tc = (T <= 256) && !getenv("SAB_NO_TC_ATTENTION");
-  if (p.att_tc) {
+  p.att_tc = !getenv("SAB_NO_TC_ATTENTION");
+  if (p.att_tc) {   // the streaming kernel (T > 256) reads Q, K and V through the 128-row box
     p.tm_att_q = make_tmap_3d(p.qkv, 3LL * d, T, Bc, 3LL * d, (int64_t)T * 3 * d, 64, 128);
-    p.tm_att_kv = make_tmap_3d(p.qkv, 3LL * d, T, Bc, 3LL * d, (int64_t)T * 3 * d, 64, 256);
+    if (T <= 256) p.tm_att_kv = make_tmap_3d(p.qkv, 3LL * d, T, Bc, 3LL * d, (int64_t)T * 3 * d, 64, 256);
   }
 
   // algorithmic FLOPs of one evaluation (GEMMs + attention), for roofline reporting
@@ -1006,6 +1007,28 @@ static void launch_attention_tc2(const CUtensorMap& tq, const CUtensorMap& tk, c
     default: throw Error(fmt("SAB_ATTN_POLY=%d not built (0, 2, 3, 4)", g_attn_poly));
   }
 #undef SAB_AT2
+}
+// wgmma streaming self-attention for T > 256 (attention_stream_tc.cuh).  shift_log2 >= 0: q is already in the log2
+// domain and every |logit| <= shift_log2 <= 50 (bounded variant, no running maximum); < 0: exact online softmax.
+template <bool kExact, int kPoly>
+static void launch_attention_stream_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                                         const AttnTc2Params& ap, cudaStream_t st) {
+  auto kern = attention_stream_tc_kernel<kExact, kPoly>;
+  ensure_dynamic_smem(reinterpret_cast<const void*>(kern), ATS_SMEM);
+  kern<<<ap.heads * ap.items * ((ap.T + 127) / 128), ATS_THREADS, ATS_SMEM, st>>>(tq, tk, tv, ap);
+  SAB_CUDA(cudaGetLastError());
+}
+static void launch_attention_stream(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                                    const AttnTc2Params& ap, cudaStream_t st) {
+  const bool exact = ap.shift_log2 < 0.f;
+  SAB_CHECK(exact || ap.shift_log2 <= 50.f, "bounded softmax needs a logit bound <= 50 (got %g)", ap.shift_log2);
+#define SAB_ATS(p_) case p_: return exact ? launch_attention_stream_inst<true, p_>(tq, tk, tv, ap, st)   \
+                                          : launch_attention_stream_inst<false, p_>(tq, tk, tv, ap, st);
+  switch (g_attn_poly) {
+    SAB_ATS(0) SAB_ATS(2) SAB_ATS(3) SAB_ATS(4)
+    default: throw Error(fmt("SAB_ATTN_POLY=%d not built (0, 2, 3, 4)", g_attn_poly));
+  }
+#undef SAB_ATS
 }
 
 // xattn_fold.cuh: every layer's Ut in one launch.  A CTA sweeps the clips in chunks whose Ut rows it holds in shared
@@ -1155,7 +1178,8 @@ static void dit_eval(sab_engine* e, const float* time_dev, const FinalSpec& fs, 
       tp.reverse = g_serpentine ? dir : 0;
       dir ^= 1;
       mark(e, st, "sdpa.self", 4.0 * Bc * H * (double)T * T * 128, (double)M * 4.0 * d * 2.0);   // reads q|k|v, writes o (bf16)
-      launch_attention_tc2(p.tm_att_q, p.tm_att_kv, p.tm_att_kv, tp, W.att_shift_log2 >= 0.f, st);
+      if (T <= 256) launch_attention_tc2(p.tm_att_q, p.tm_att_kv, p.tm_att_kv, tp, W.att_shift_log2 >= 0.f, st);
+      else launch_attention_stream(p.tm_att_q, p.tm_att_q, p.tm_att_q, tp, st);
     } else {
       attention(e, a, Bc, H, st);
     }
@@ -1206,6 +1230,7 @@ struct CodecPlan {
   bf16* z_in = nullptr;                                  // decoder input [items, T, cz] bf16
   bf16* a_last = nullptr;                                // decoder last-stage activated input
   GemmOp* enc_out = nullptr;                             // in_proj (output pointer patched per chunk)
+  float* tile_in = nullptr; float* tile_out = nullptr;   // time-tiled clips: one tile's input and output (allocated on first use)
   double flops = 0;
   int64_t last_use = 0;
 };
@@ -1845,15 +1870,73 @@ static void run_codec(sab_engine* e, CodecPlan& cp, int items, const float* wav_
   SAB_CUDA(cudaGetLastError());
 }
 
-static int codec_chunk(const sab_engine* e, long long S_samples, bool decoder) {
-  // fp32 stream + two bf16 operand buffers per stage (8 B per activation element): ~0.56 GB per 10 s clip in the
-  // encoder, ~0.85 GB per 10 s waveform in the decoder; keep a chunk's workspace near 12 GB
-  (void)e;
-  const double per_item = (double)S_samples / 480000.0 * (decoder ? 0.85e9 : 0.56e9);
-  double budget = 12e9;
-  if (const char* b = getenv("SAB_CODEC_CHUNK_BYTES")) budget = atof(b);   // tests force small chunks through this
-  int n = (int)(budget / per_item);
+// Workspace of one codec item by the planner's constants (fp32 stream + two bf16 operand buffers per stage, 8 B per
+// activation element): ~0.56 GB per 10 s clip in the encoder, ~0.85 GB per 10 s waveform in the decoder.
+static double codec_item_bytes(long long S_samples, bool decoder) {
+  return (double)S_samples / 480000.0 * (decoder ? 0.85e9 : 0.56e9);
+}
+static double codec_budget() {   // a chunk's workspace stays near 12 GB
+  if (const char* b = getenv("SAB_CODEC_CHUNK_BYTES")) return atof(b);   // tests force small chunks and tiles through this
+  return 12e9;
+}
+static int codec_chunk(long long S_samples, bool decoder) {
+  const int n = (int)(codec_budget() / codec_item_bytes(S_samples, decoder));
   return n < 1 ? 1 : (n > 64 ? 64 : n);
+}
+
+// ---- time tiling of clips that do not fit the budget whole ----
+// The codec is local in time (convolutions, Snake, tanh), so an output frame depends on a bounded window of input
+// frames.  The window's half-width ("halo", in latent frames) follows from the layer list: walking from the output
+// back to the input, a Conv1d(k, dilation) widens the context by (k - 1) / 2 * dilation samples, a stride-s
+// Conv1d(k = 2s) reads the input rows -1 .. +1 of its [T / s, s * C] view and a ConvTranspose1d(k = 2s, stride s) the
+// input rows -1 .. +1 of each output row.
+static long long conv_ctx(long long r, const ConvLayer& L) { return r + (long long)((L.k - 1) / 2) * L.dil; }
+static int codec_halo_frames(const sab_engine* e, bool decoder) {
+  const sab_config& c = e->cfg;
+  long long r = 0;
+  if (decoder) {                                     // waveform samples back to latent frames
+    r += 3;                                          // dec.last: 7 taps (dec_last_reg_kernel)
+    for (int i = c.codec_n_rates - 1; i >= 0; --i) {
+      const DecBlockW& B = e->dec_blocks[i];
+      for (int j = 2; j >= 0; --j) r = conv_ctx(conv_ctx(r, B.ru[j].c1), B.ru[j].c7);
+      r = (r + B.stride - 1) / B.stride + 1;
+    }
+    return (int)conv_ctx(r, e->dec0);                // out_proj is 1 x 1
+  }
+  long long hop = 1;                                 // latent frames back to waveform samples
+  r = conv_ctx(r, e->enc_final);                     // in_proj is 1 x 1
+  for (int i = c.codec_n_rates - 1; i >= 0; --i) {
+    const EncBlockW& B = e->enc_blocks[i];
+    r = (r + 1) * B.stride;
+    for (int j = 2; j >= 0; --j) r = conv_ctx(conv_ctx(r, B.ru[j].c1), B.ru[j].c7);
+    hop *= B.stride;
+  }
+  r += 3;                                            // enc.conv0: 7 taps (enc_conv0_reg_kernel)
+  return (int)((r + hop - 1) / hop);
+}
+// Tiles of Lt latent frames over a clip of T > Lt frames.  Tile {start, w0, w1} is computed over [start, start + Lt)
+// and its rows [w0, w1) are kept: at least `halo` computed rows lie between a kept row and an interior tile edge, and
+// the first and last tile end at the clip's edges, where the plan's zero fill is the convolution padding as in an
+// un-tiled run.  The last tile is right-aligned, so every tile has the plan's length.
+struct CodecTile { int start, w0, w1; };
+static std::vector<CodecTile> codec_tiles(int T, int Lt, int halo) {
+  std::vector<CodecTile> tiles;
+  int w0 = 0;
+  for (;;) {
+    const int start = w0 == 0 ? 0 : w0 - halo;
+    if (start + Lt >= T) { tiles.push_back({T - Lt, w0, T}); return tiles; }
+    tiles.push_back({start, w0, start + Lt - halo});
+    w0 = start + Lt - halo;
+  }
+}
+// tile length in latent frames for a clip that does not fit the budget as `min_items` whole items; 0: run it whole
+static int codec_tile_frames(const sab_engine* e, int T, long long hop, bool decoder) {
+  const int min_items = decoder ? 2 : 1;
+  if (codec_budget() >= min_items * codec_item_bytes((long long)T * hop, decoder)) return 0;
+  const int halo = codec_halo_frames(e, decoder);
+  int Lt = (int)(codec_budget() / (min_items * codec_item_bytes(hop, decoder)));
+  Lt = std::max(Lt, 4 * halo);                       // at least half of a tile is kept
+  return Lt < T ? Lt : 0;
 }
 
 int sab_encode(sab_engine* e, const float* wav, int B, int64_t S, float* features, void* stream) {
@@ -1864,12 +1947,26 @@ int sab_encode(sab_engine* e, const float* wav, int B, int64_t S, float* feature
   for (int i = 0; i < e->cfg.codec_n_rates; ++i) hop *= e->cfg.codec_encoder_rates[i];
   SAB_CHECK(S % hop == 0, "S=%lld must be padded to a multiple of hop=%lld (codec.py:72-78)", (long long)S, hop);
   const long long T = S / hop;
-  const int chunk = std::min(B, codec_chunk(e, S, false));
-  CodecPlan* cp = get_enc_plan(e, chunk, S);
-  for (int b0 = 0; b0 < B; b0 += chunk) {
-    const int n = std::min(chunk, B - b0);
-    run_codec(e, *cp, n, wav + (long long)b0 * S, nullptr, (int)T,
-              features + (long long)b0 * T * 2 * e->cfg.codec_codebook_dim, st);
+  const int cf = 2 * e->cfg.codec_codebook_dim;
+  if (const int Lt = codec_tile_frames(e, (int)T, hop, false)) {
+    // one tile at a time through a plan of tile length; the two ends are staged so that the plan runs unchanged
+    CodecPlan* cp = get_enc_plan(e, 1, Lt * hop);
+    if (!cp->tile_in) { cp->tile_in = cp->pool.alloc<float>(Lt * hop); cp->tile_out = cp->pool.alloc<float>((int64_t)Lt * cf); }
+    const auto tiles = codec_tiles((int)T, Lt, codec_halo_frames(e, false));
+    for (int b = 0; b < B; ++b)
+      for (const CodecTile& t : tiles) {
+        SAB_CUDA(cudaMemcpyAsync(cp->tile_in, wav + b * S + t.start * hop, Lt * hop * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        run_codec(e, *cp, 1, cp->tile_in, nullptr, Lt, cp->tile_out, st);
+        SAB_CUDA(cudaMemcpyAsync(features + (b * T + t.w0) * cf, cp->tile_out + (int64_t)(t.w0 - t.start) * cf,
+                                 (int64_t)(t.w1 - t.w0) * cf * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      }
+  } else {
+    const int chunk = std::min(B, codec_chunk(S, false));
+    CodecPlan* cp = get_enc_plan(e, chunk, S);
+    for (int b0 = 0; b0 < B; b0 += chunk) {
+      const int n = std::min(chunk, B - b0);
+      run_codec(e, *cp, n, wav + (long long)b0 * S, nullptr, (int)T, features + (long long)b0 * T * cf, st);
+    }
   }
   SAB_API_END
 }
@@ -1882,16 +1979,43 @@ int sab_decode(sab_engine* e, const float* latent, int Bc, int T, float* wav, vo
   for (int i = 0; i < e->cfg.codec_n_rates; ++i) hop *= e->cfg.codec_decoder_rates[i];
   const long long S = (long long)T * hop;
   const int items = 2 * Bc;
-  // whole clips per chunk: items (2b, 2b+1) = (target, residual) come from the two halves of latent row b, so a chunk
-  // is always an even number of items, at least one clip (a single-item chunk would decode the target half twice)
-  int chunk = std::min(items, std::max(2, codec_chunk(e, S, true) & ~1));
-  CodecPlan* cp = get_dec_plan(e, chunk, T);
   const int cz = e->cfg.codec_codebook_dim;
-  for (int i0 = 0; i0 < items; i0 += chunk) {
-    const int n = std::min(chunk, items - i0);
-    // items (2b, 2b+1) live in latent row b: chunk boundaries are clip boundaries
-    run_codec(e, *cp, n, nullptr, latent + (long long)(i0 / 2) * T * 2 * cz, T, wav + (long long)i0 * S, st);
+  if (const int Lt = codec_tile_frames(e, T, hop, true)) {
+    // one tile of one clip at a time: the tile's latent rows [Lt, 2 cz] split into the (target, residual) item pair
+    // exactly as a whole clip's do
+    CodecPlan* cp = get_dec_plan(e, 2, Lt);
+    if (!cp->tile_in) { cp->tile_in = cp->pool.alloc<float>((int64_t)Lt * 2 * cz); cp->tile_out = cp->pool.alloc<float>(2 * Lt * hop); }
+    const auto tiles = codec_tiles(T, Lt, codec_halo_frames(e, true));
+    for (int b = 0; b < Bc; ++b)
+      for (const CodecTile& t : tiles) {
+        SAB_CUDA(cudaMemcpyAsync(cp->tile_in, latent + ((long long)b * T + t.start) * 2 * cz, (int64_t)Lt * 2 * cz * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, st));
+        run_codec(e, *cp, 2, nullptr, cp->tile_in, Lt, cp->tile_out, st);
+        for (int half = 0; half < 2; ++half)
+          SAB_CUDA(cudaMemcpyAsync(wav + (2LL * b + half) * S + t.w0 * hop, cp->tile_out + half * Lt * hop + (t.w0 - t.start) * hop,
+                                   (t.w1 - t.w0) * hop * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      }
+  } else {
+    // whole clips per chunk: items (2b, 2b+1) = (target, residual) come from the two halves of latent row b, so a chunk
+    // is always an even number of items, at least one clip (a single-item chunk would decode the target half twice)
+    int chunk = std::min(items, std::max(2, codec_chunk(S, true) & ~1));
+    CodecPlan* cp = get_dec_plan(e, chunk, T);
+    for (int i0 = 0; i0 < items; i0 += chunk) {
+      const int n = std::min(chunk, items - i0);
+      // items (2b, 2b+1) live in latent row b: chunk boundaries are clip boundaries
+      run_codec(e, *cp, n, nullptr, latent + (long long)(i0 / 2) * T * 2 * cz, T, wav + (long long)i0 * S, st);
+    }
   }
+  SAB_API_END
+}
+
+int sab_codec_tiling(sab_engine* e, int decoder, int T, int* halo_frames, int* tile_frames) {
+  SAB_API_BEGIN_E(e)
+  SAB_CHECK(e->finalized && halo_frames && tile_frames && T > 0, "bad argument");
+  long long hop = 1;
+  for (int i = 0; i < e->cfg.codec_n_rates; ++i) hop *= decoder ? e->cfg.codec_decoder_rates[i] : e->cfg.codec_encoder_rates[i];
+  *halo_frames = codec_halo_frames(e, decoder != 0);
+  *tile_frames = codec_tile_frames(e, T, hop, decoder != 0);
   SAB_API_END
 }
 
@@ -2098,6 +2222,32 @@ int sab_test_attention_tc2(int items, int heads, int T, const void* q, const voi
     // shift_log2 == 0: folded path (the caller passes q already multiplied by log2(e)/sqrt(hd), |logit| <= 50)
     if (shift_log2 == 0.f) tp.shift_log2 = 50.f;
     launch_attention_tc2(tq, tk, tv, tp, shift_log2 == 0.f, (cudaStream_t)stream);
+  } catch (...) {
+    g_attn_poly = saved;
+    throw;
+  }
+  g_attn_poly = saved;
+  SAB_API_END
+}
+
+int sab_test_attention_stream(int items, int heads, int T, const void* q, const void* k, const void* v,
+                              const uint8_t* key_mask, void* o, float shift_log2, int poly, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(T >= 1 && items >= 1 && heads >= 1, "bad shape");
+  const long long ld = (long long)heads * 128;
+  CUtensorMap tq = make_tmap_3d(q, ld, T, items, ld, (int64_t)T * ld, 64, 128);
+  CUtensorMap tk = make_tmap_3d(k, ld, T, items, ld, (int64_t)T * ld, 64, 128);
+  CUtensorMap tv = make_tmap_3d(v, ld, T, items, ld, (int64_t)T * ld, 64, 128);
+  AttnTc2Params tp{};
+  tp.o = (bf16*)o; tp.o_ld = ld;
+  tp.key_mask = key_mask; tp.T = T; tp.heads = heads; tp.items = items; tp.mask_div = 1;
+  tp.q_col0 = tp.k_col0 = tp.v_col0 = 0;
+  tp.scale_log2 = (1.0f / sqrtf(128.f)) * 1.4426950408889634f;   // exact variant; the bounded one takes q pre-scaled
+  tp.shift_log2 = shift_log2 == 0.f ? 50.f : shift_log2;
+  const int saved = g_attn_poly;
+  if (poly >= 0) g_attn_poly = poly;
+  try {
+    launch_attention_stream(tq, tk, tv, tp, (cudaStream_t)stream);
   } catch (...) {
     g_attn_poly = saved;
     throw;
