@@ -240,6 +240,19 @@ int sab_codec_tiling(sab_engine* e, int decoder, int T, int* halo_frames, int* t
  * Engine-independent (no weights). */
 int sab_preprocess_frames(const uint8_t* frames, int n_frames, int H, int W, int out_size, float* workspace, float* out,
                           void* stream);
+/* Long recordings, cross-fade of overlapping windows.  replaces: nothing — the reference has no windowing (its RoPE table
+ * ends at max_positions, rope.py:152); SAMAudio.separate() solves a batch longer than the table as windows of Tw frames
+ * and blends them with this (DESIGN.md section 3).  Engine-independent (no weights).
+ *  win_latent [n_win, Tw, 256] fp32; per window (device arrays): win_seq = destination sequence in [0, Bc),
+ *  win_start = its first frame, win_flags = SAB_WIN_FIRST | SAB_WIN_LAST (first / last window of its clip);
+ *  latent [Bc, T, 256] fp32 out, every frame written:
+ *    latent[s, t] = sum_k w_k x_k[t - start_k] / sum_k w_k over the windows k of s covering t, ascending k, fp32;
+ *    w = min(ramp_in, ramp_out) at local position j, ramp_in = min(1, (j + 0.5) / ramp) (1 for a first window),
+ *    ramp_out = min(1, (Tw - j - 0.5) / ramp) (1 for a last window); frames no window covers are 0. */
+#define SAB_WIN_FIRST 1
+#define SAB_WIN_LAST 2
+int sab_blend_windows(const float* win_latent, int n_win, int Tw, const int32_t* win_seq, const int32_t* win_start,
+                      const uint8_t* win_flags, int ramp, float* latent, int Bc, int T, void* stream);
 /* host-only test seam: evaluation times of sab_solve's grid (method = SAB_ODE_*), in evaluation order */
 int sab_test_solver_grid(int method, int n_steps, int cap, int* n_evals, float* times);
 /* host-only test seam: tap window start / count / normalised weights ([out_size, cap], zero padded) of one axis */

@@ -83,7 +83,7 @@ class SabTestGemmDesc(ctypes.Structure):
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
-    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_blend_windows", "sab_test_aa_taps", "sab_test_solver_grid",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -126,6 +126,7 @@ def lib() -> ctypes.CDLL:
         L.sab_test_attention_stream.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, ctypes.c_float, i32, vp]
         L.sab_codec_tiling.argtypes = [vp, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32)]
         L.sab_preprocess_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
+        L.sab_blend_windows.argtypes = [vp, i32, i32, vp, vp, vp, i32, vp, i32, i32, vp]
         L.sab_test_aa_taps.argtypes = [i32, i32, i32, vp, vp, vp, vp]
         L.sab_test_solver_grid.argtypes = [i32, i32, i32, vp, vp]
         L.sab_t5_create.argtypes = [ctypes.POINTER(SabT5Config), i32, ctypes.POINTER(vp)]
@@ -184,6 +185,26 @@ def preprocess_frames(frames: torch.Tensor, out_size: int) -> torch.Tensor:
     ws = torch.empty(n, 3, h, out_size, device=frames.device, dtype=torch.float32)
     with torch.cuda.device(frames.device):
         check(lib().sab_preprocess_frames(frames.data_ptr(), n, h, w, out_size, ws.data_ptr(), out.data_ptr(), stream_ptr()))
+    return out
+
+
+WIN_FIRST, WIN_LAST = 1, 2   # include/samaudio_b200.h SAB_WIN_*
+
+
+def blend_windows(win_latent: torch.Tensor, seq: torch.Tensor, start: torch.Tensor, flags: torch.Tensor, ramp: int,
+                  out: torch.Tensor) -> torch.Tensor:
+    """win_latent [n_win, Tw, 256] fp32 -> out [Bc, T, 256]: the cross-fade of sab_blend_windows (all tensors on one
+    device; seq / start int32, flags uint8 = WIN_FIRST | WIN_LAST, one entry per window)."""
+    n_win, Tw, C = win_latent.shape
+    Bc, T, C2 = out.shape
+    assert C == C2 == 256 and win_latent.dtype == out.dtype == torch.float32
+    assert win_latent.is_contiguous() and out.is_contiguous()
+    assert seq.dtype == start.dtype == torch.int32 and flags.dtype == torch.uint8
+    assert seq.shape == start.shape == flags.shape == (n_win,)
+    seq, start, flags = seq.contiguous(), start.contiguous(), flags.contiguous()
+    with torch.cuda.device(out.device):
+        check(lib().sab_blend_windows(win_latent.data_ptr(), n_win, Tw, seq.data_ptr(), start.data_ptr(),
+                                      flags.data_ptr(), int(ramp), out.data_ptr(), Bc, T, stream_ptr()))
     return out
 
 

@@ -20,6 +20,7 @@
 #include "codec_kernels.cuh"
 #include "vision_kernels.cuh"
 #include "xattn_fold.cuh"
+#include "blend_windows.cuh"
 
 using namespace sab;
 typedef __nv_bfloat16 bf16;
@@ -780,6 +781,10 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
   const int64_t M = (int64_t)Bc * T, MB = (int64_t)B * T, ML = (int64_t)B * L;
   p.M = M; p.MB = MB; p.ML = ML;
   SAB_CHECK(T <= e->rope_len, "T=%d exceeds the RoPE table (%d)", T, e->rope_len);
+  // the DiT kernels count rows (sequence x frame) in 32-bit integers (dit_eval's M, rmsnorm_mod_kernel,
+  // cond_finish_kernel, the GEMM's row indices); element offsets are 64-bit
+  SAB_CHECK(M <= INT32_MAX - 256, "%lld DiT rows (B*candidates=%d x T=%d) exceed the 32-bit row index", (long long)M, Bc,
+            T);
   DevicePool& w = p.pool;
   p.y = w.alloc<float>(M * 256); p.ymid = w.alloc<float>(M * 256);
   p.cond = w.alloc<float>(M * d); p.x0 = w.alloc<float>(M * d); p.c1 = w.alloc<float>(M * d);
@@ -2348,6 +2353,19 @@ int sab_preprocess_frames(const uint8_t* frames, int n_frames, int H, int W, int
   const int planes = n_frames * 3;
   resize_rows_kernel<<<dim3(H, planes), 256, W, st>>>(frames, H, W, out_size, tx.lo, tx.cnt, tx.w, tx.taps, workspace);
   resize_cols_finish_kernel<<<dim3(out_size, planes), 256, 0, st>>>(workspace, H, out_size, ty.lo, ty.cnt, ty.w, ty.taps, out);
+  SAB_CUDA(cudaGetLastError());
+  SAB_API_END
+}
+
+int sab_blend_windows(const float* win_latent, int n_win, int Tw, const int32_t* win_seq, const int32_t* win_start,
+                      const uint8_t* win_flags, int ramp, float* latent, int Bc, int T, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(win_latent && win_seq && win_start && win_flags && latent, "null argument");
+  SAB_CHECK(n_win >= 1 && Tw >= 1 && ramp >= 1 && T >= 1, "bad shape (n_win=%d, Tw=%d, ramp=%d, T=%d)", n_win, Tw, ramp, T);
+  SAB_CHECK(Bc >= 1 && Bc <= 65535, "Bc=%d outside 1..65535", Bc);
+  BlendParams bp{win_latent, win_seq, win_start, win_flags, n_win, Tw, ramp, latent, T};
+  const int per_cta = BW_WARPS * BW_FRAMES;
+  blend_windows_kernel<<<dim3((T + per_cta - 1) / per_cta, Bc), BW_WARPS * 32, 0, (cudaStream_t)stream>>>(bp);
   SAB_CUDA(cudaGetLastError());
   SAB_API_END
 }

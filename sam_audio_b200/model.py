@@ -274,16 +274,23 @@ class SAMAudio(torch.nn.Module):
         anchor_ids, anchor_alignment, pad_mask = batch.anchor_ids, batch.anchor_alignment, batch.audio_pad_mask
         if predict_spans and getattr(self, "span_predictor", None) is not None and batch.anchors is None:
             batch = self.predict_spans(batch, feats, batch.audio_pad_mask)
-        self._install_conditioning(feats, text_features, text_mask, video, anchor_ids, anchor_alignment, pad_mask,
-                                   candidates=c)
+        # a batch longer than the model's position table is solved as overlapping windows (sam_audio_b200.windows)
+        windowed = T > self.cfg.transformer.max_positions
+        if not windowed:
+            self._install_conditioning(feats, text_features, text_mask, video, anchor_ids, anchor_alignment, pad_mask,
+                                       candidates=c)
         if noise is None:
             noise = torch.randn(B * c, T, C2, device=feats.device, dtype=torch.float32)
         noise = noise.to(device=feats.device, dtype=torch.float32).contiguous()
-        latent = torch.empty_like(noise)
         hop = self.cfg.audio_codec.hop_length
         wavs = torch.empty(B * c, 2, T * hop, device=feats.device, dtype=torch.float32)
         with torch.cuda.device(feats.device):
-            eng.solve(noise, n_steps, latent, method)
+            if windowed:
+                latent = self._solve_windows(feats, text_features, text_mask, video, anchor_ids, anchor_alignment,
+                                             pad_mask, batch.sizes, noise, c, n_steps, method)
+            else:
+                latent = torch.empty_like(noise)
+                eng.solve(noise, n_steps, latent, method)
             if _on_decoded is None:
                 eng.decode(latent, B * c, T, wavs)
             else:                                                           # whole clips (all candidates) per chunk
@@ -313,6 +320,44 @@ class SAMAudio(torch.nn.Module):
         idxs = [int(i) for i in idxs]
         return SeparationResult(target=[w[i] for w, i in zip(tgt, idxs)],
                                 residual=[w[i] for w, i in zip(res, idxs)], noise=noise)
+
+    def _solve_windows(self, feats, text_features, text_mask, video, anchor_ids, anchor_alignment, pad_mask, sizes,
+                       noise, c: int, n_steps: int, method: str) -> torch.Tensor:
+        """The ODE solve of a batch longer than the position table: every clip is cut into windows of max_positions
+        frames (window_layout), the windows are solved in groups of bounded size as clips of their own, and their
+        latents are cross-faded on the device into latent [B * c, T, 256].  A window's inputs are copies of its clip's
+        frames (text, text mask and anchor ids: the clip's own), its noise rows are noise[clip * c + k, start:start + Tw],
+        so overlapping windows start from the same noise there."""
+        from .windows import window_groups, window_layout, window_ramp, window_rows_budget
+        eng = self._ensure_engine()
+        B, T, C2 = feats.shape
+        Tw = self.cfg.transformer.max_positions
+        dev = feats.device
+        wins = window_layout([int(n) for n in sizes], Tw)
+        noise_bc = noise.view(B, c, T, C2)
+        win_lat = torch.empty(len(wins) * c, Tw, C2, device=dev, dtype=torch.float32)   # window-major, candidate-minor
+        for i, w in enumerate(wins):
+            win_lat[i * c:(i + 1) * c] = noise_bc[w.clip, :, w.start:w.start + Tw]
+
+        def cut(x, time_dim=1):           # [B, T, ...] (or [B, C, T]) -> the group's windows
+            if x is None:
+                return None
+            return torch.stack([x[w.clip].narrow(time_dim - 1, w.start, Tw) for w in grp])
+
+        def per_clip(x):                  # the clip's own row, once per window
+            return None if x is None else torch.stack([x[w.clip] for w in grp])
+        for w0, w1 in window_groups(len(wins), c, Tw, window_rows_budget()):
+            grp = wins[w0:w1]
+            self._install_conditioning(cut(feats), per_clip(text_features), per_clip(text_mask), cut(video, 2),
+                                       per_clip(anchor_ids), cut(anchor_alignment), cut(pad_mask), candidates=c)
+            rows = win_lat[w0 * c:w1 * c]
+            eng.solve(rows, n_steps, rows, method)
+        seq = torch.tensor([w.clip * c + k for w in wins for k in range(c)], dtype=torch.int32)
+        start = torch.tensor([w.start for w in wins for _ in range(c)], dtype=torch.int32)
+        flags = torch.tensor([_capi.WIN_FIRST * w.first + _capi.WIN_LAST * w.last for w in wins for _ in range(c)],
+                             dtype=torch.uint8)
+        latent = torch.empty(B * c, T, C2, device=dev, dtype=torch.float32)
+        return _capi.blend_windows(win_lat, seq.to(dev), start.to(dev), flags.to(dev), window_ramp(Tw), latent)
 
     def predict_spans(self, batch: Batch, audio_features: torch.Tensor, audio_pad_mask: torch.Tensor) -> Batch:
         """Reference model.py:231-245: frame-level span predictor on the first 128 latent channels -> "+" anchors ->
