@@ -245,6 +245,8 @@ int sab_preprocess_frames(const uint8_t* frames, int n_frames, int H, int W, int
  * and blends them with this (DESIGN.md section 3).  Engine-independent (no weights).
  *  win_latent [n_win, Tw, 256] fp32; per window (device arrays): win_seq = destination sequence in [0, Bc),
  *  win_start = its first frame, win_flags = SAB_WIN_FIRST | SAB_WIN_LAST (first / last window of its clip);
+ *  starts may be negative or past T, so latent can be a frame range of a longer timeline (streams pass starts relative
+ *  to the first frame they blend);
  *  latent [Bc, T, 256] fp32 out, every frame written:
  *    latent[s, t] = sum_k w_k x_k[t - start_k] / sum_k w_k over the windows k of s covering t, ascending k, fp32;
  *    w = min(ramp_in, ramp_out) at local position j, ramp_in = min(1, (j + 0.5) / ramp) (1 for a first window),

@@ -56,6 +56,23 @@ def fold_weight_norm(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Ten
     return out
 
 
+def _ode_grid(ode_opt: Dict[str, Any]):
+    """(n_steps, method) of a fixed-grid `ode_opt`.  The reference forwards **ode_opt to torchdiffeq.odeint
+    (model.py:285-290); its fixed-grid solvers are built."""
+    method = ode_opt.get("method", "midpoint")
+    if method not in _capi.Engine.ODE_METHODS:
+        raise NotImplementedError(f"ode method {method!r}: the fixed-grid solvers {sorted(_capi.Engine.ODE_METHODS)} "
+                                  "are implemented (adaptive torchdiffeq solvers are not)")
+    step = ode_opt.get("options", {}).get("step_size")
+    if step is None:
+        raise NotImplementedError("fixed-grid solvers need options={'step_size': ...} (torchdiffeq would otherwise "
+                                  "take ONE step over [0, 1])")
+    n_steps = round(1.0 / float(step))
+    if abs(n_steps * float(step) - 1.0) > 1e-6:
+        raise NotImplementedError(f"step_size {step} does not divide [0, 1]")
+    return n_steps, method
+
+
 class SAMAudio(torch.nn.Module):
     config_cls = SAMAudioConfig
     revision = None
@@ -245,18 +262,7 @@ class SAMAudio(torch.nn.Module):
         """`_on_decoded(i0, i1, wavs)` (private; sam_audio_b200.parallel): called after the waveforms of sequences
         [i0, i1) are enqueued for decoding, so that a collective on them can overlap the next chunk's decode."""
         c = int(reranking_candidates)
-        # the reference forwards **ode_opt to torchdiffeq.odeint (model.py:285-290); its fixed-grid solvers are built
-        method = ode_opt.get("method", "midpoint")
-        if method not in _capi.Engine.ODE_METHODS:
-            raise NotImplementedError(f"ode method {method!r}: the fixed-grid solvers {sorted(_capi.Engine.ODE_METHODS)} "
-                                      "are implemented (adaptive torchdiffeq solvers are not)")
-        step = ode_opt.get("options", {}).get("step_size")
-        if step is None:
-            raise NotImplementedError("fixed-grid solvers need options={'step_size': ...} (torchdiffeq would otherwise "
-                                      "take ONE step over [0, 1])")
-        n_steps = round(1.0 / float(step))
-        if abs(n_steps * float(step) - 1.0) > 1e-6:
-            raise NotImplementedError(f"step_size {step} does not divide [0, 1]")
+        n_steps, method = _ode_grid(ode_opt)
         eng = self._ensure_engine()
 
         feats = self._get_audio_features(batch.audios)                      # [B, T, 256]
@@ -286,8 +292,11 @@ class SAMAudio(torch.nn.Module):
         wavs = torch.empty(B * c, 2, T * hop, device=feats.device, dtype=torch.float32)
         with torch.cuda.device(feats.device):
             if windowed:
+                from .windows import window_layout
+                Tw = self.cfg.transformer.max_positions
                 latent = self._solve_windows(feats, text_features, text_mask, video, anchor_ids, anchor_alignment,
-                                             pad_mask, batch.sizes, noise, c, n_steps, method)
+                                             pad_mask, window_layout([int(n) for n in batch.sizes], Tw), Tw, noise, c,
+                                             n_steps, method)
             else:
                 latent = torch.empty_like(noise)
                 eng.solve(noise, n_steps, latent, method)
@@ -321,19 +330,18 @@ class SAMAudio(torch.nn.Module):
         return SeparationResult(target=[w[i] for w, i in zip(tgt, idxs)],
                                 residual=[w[i] for w, i in zip(res, idxs)], noise=noise)
 
-    def _solve_windows(self, feats, text_features, text_mask, video, anchor_ids, anchor_alignment, pad_mask, sizes,
-                       noise, c: int, n_steps: int, method: str) -> torch.Tensor:
-        """The ODE solve of a batch longer than the position table: every clip is cut into windows of max_positions
-        frames (window_layout), the windows are solved in groups of bounded size as clips of their own, and their
-        latents are cross-faded on the device into latent [B * c, T, 256].  A window's inputs are copies of its clip's
-        frames (text, text mask and anchor ids: the clip's own), its noise rows are noise[clip * c + k, start:start + Tw],
-        so overlapping windows start from the same noise there."""
-        from .windows import window_groups, window_layout, window_ramp, window_rows_budget
+    def _solve_windows(self, feats, text_features, text_mask, video, anchor_ids, anchor_alignment, pad_mask, wins,
+                       Tw: int, noise, c: int, n_steps: int, method: str) -> torch.Tensor:
+        """The ODE solve of a batch cut into windows of Tw frames (`wins`, a list of windows.Window; separate() passes
+        window_layout(sizes, max_positions)): the windows are solved in groups of bounded size as clips of their own,
+        and their latents are cross-faded on the device into latent [B * c, T, 256].  A window's inputs are copies of
+        its clip's frames (text, text mask and anchor ids: the clip's own), its noise rows are
+        noise[clip * c + k, start:start + Tw], so overlapping windows start from the same noise there.  Every window
+        must lie inside [0, T)."""
+        from .windows import window_groups, window_ramp, window_rows_budget
         eng = self._ensure_engine()
         B, T, C2 = feats.shape
-        Tw = self.cfg.transformer.max_positions
         dev = feats.device
-        wins = window_layout([int(n) for n in sizes], Tw)
         noise_bc = noise.view(B, c, T, C2)
         win_lat = torch.empty(len(wins) * c, Tw, C2, device=dev, dtype=torch.float32)   # window-major, candidate-minor
         for i, w in enumerate(wins):
@@ -358,6 +366,36 @@ class SAMAudio(torch.nn.Module):
                              dtype=torch.uint8)
         latent = torch.empty(B * c, T, C2, device=dev, dtype=torch.float32)
         return _capi.blend_windows(win_lat, seq.to(dev), start.to(dev), flags.to(dev), window_ramp(Tw), latent)
+
+    def stream(self, description: str, window_seconds: float = 10.0, seed: int = 0,
+               ode_opt: Dict[str, Any] = DFLT_ODE_OPT, reranking_candidates: int = 1, anchors=None,
+               masked_video=None):
+        """Separation of audio that arrives in chunks (sam_audio_b200.stream, DESIGN.md section 3):
+
+            s = model.stream(description="man speaking")
+            for chunk in source:          # [S] or [1, S] float samples at the model's rate, any S >= 1
+                out = s.push(chunk)       # out.target / out.residual: the samples that became final
+            tail = s.flush()              # the rest; the stream is closed afterwards
+
+        The stream is solved as windows of W = round(window_seconds * 25) latent frames, 8 <= W <= max_positions; the
+        default 10 s keeps the DiT on its short-sequence attention (T <= 256).  Text prompts with one candidate only."""
+        from .stream import SeparationStream
+        from .windows import stream_window_frames
+        cc = self.cfg.audio_codec
+        W = stream_window_frames(window_seconds, cc.sample_rate / cc.hop_length, self.cfg.transformer.max_positions)
+        if int(reranking_candidates) != 1:
+            raise NotImplementedError("a stream has one candidate: the rankers that choose among candidates score whole "
+                                      "clips, which a stream never holds")
+        if anchors is not None:
+            raise NotImplementedError("a stream takes no anchors: anchor spans are times in a clip, and a stream has no "
+                                      "time base for them yet")
+        if masked_video is not None:
+            raise NotImplementedError("a stream takes no masked video: video frames would need a time base aligned with "
+                                      "the stream, which it does not have yet")
+        if not isinstance(description, str):
+            raise TypeError("a stream separates one source: description must be one string")
+        n_steps, method = _ode_grid(ode_opt)
+        return SeparationStream(self, description, W, int(seed), n_steps, method)
 
     def predict_spans(self, batch: Batch, audio_features: torch.Tensor, audio_pad_mask: torch.Tensor) -> Batch:
         """Reference model.py:231-245: frame-level span predictor on the first 128 latent channels -> "+" anchors ->

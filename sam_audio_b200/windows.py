@@ -3,7 +3,8 @@
 The DiT's RoPE table ends at ``transformer.max_positions`` frames (reference rope.py:152), so ``SAMAudio.separate()``
 solves a longer batch as overlapping windows of exactly that length and cross-fades their latents on the device
 (``sab_blend_windows``).  This module is the integer part: where the windows start and how they are grouped into
-solves of bounded size.  Pure host logic, shared by ``separate()`` and the tests.
+solves of bounded size, for ``separate()`` and for streams (``SAMAudio.stream()``), whose layout must not depend on
+samples that have not arrived.  Pure host logic, shared by the model and the tests.
 """
 from __future__ import annotations
 
@@ -48,6 +49,59 @@ def window_layout(sizes: Sequence[int], Tw: int) -> List[Window]:
         starts = clip_window_starts(int(n), Tw)
         out += [Window(b, s, i == 0, i == len(starts) - 1) for i, s in enumerate(starts)]
     return out
+
+
+# ---- streams (SAMAudio.stream, DESIGN.md section 3) ----
+# A stream does not know its length until flush(), so its windows cannot be spread over it: window k starts at k * H with
+# H = W - O, whatever the length, and flush() adds windows until the last valid frame is covered.  Every window a stream
+# has solved before flush() is therefore one of the windows of the final layout.
+
+
+def stream_hop(W: int) -> int:
+    """Frames between the starts of adjacent stream windows: W - window_ramp(W), so adjacent windows overlap by
+    exactly window_ramp(W) frames."""
+    return int(W) - window_ramp(W)
+
+
+def stream_window_starts(n_final: int, W: int) -> List[int]:
+    """Start frames of every window of a stream of n_final valid frames after flush(): k * H for the fewest k = 0, 1, ...
+    whose windows cover [0, n_final), at least one.  The last window may run past n_final (padding, masked)."""
+    n, W, H = max(1, int(n_final)), int(W), stream_hop(W)
+    return [k * H for k in range(1 + max(0, -(-(n - W) // H)))]
+
+
+def stream_frames_available(n_samples: int, hop: int, halo_enc: int) -> int:
+    """Latent frames [0, result) the codec encoder can produce, before flush(), from the first n_samples samples: a frame
+    needs halo_enc frames of samples past its own end."""
+    return max(0, int(n_samples) // int(hop) - int(halo_enc))
+
+
+def stream_windows_ready(n_frames: int, W: int) -> int:
+    """Windows that can be solved, before flush(), once frames [0, n_frames) are encoded: those with k * H + W <= n."""
+    n, W = int(n_frames), int(W)
+    return 0 if n < W else (n - W) // stream_hop(W) + 1
+
+
+def stream_final_frames(n_solved: int, W: int, n_final: int = -1) -> int:
+    """Frames [0, result) whose latent is final once windows [0, n_solved) are solved.  Before flush() (n_final < 0) frame
+    t is final when window t // H, the last window that can cover it, is solved; after flush() every window of
+    stream_window_starts(n_final, W) is solved and all n_final frames are final."""
+    return int(n_final) if n_final >= 0 else int(n_solved) * stream_hop(W)
+
+
+def stream_emit_end(final: int, halo_dec: int, flushed: bool) -> int:
+    """Frames [0, result) that can be decoded to audio: a frame needs halo_dec final frames past it, except at the end of
+    the stream, where the decoder's zero fill is the clip edge."""
+    return int(final) if flushed else max(0, int(final) - int(halo_dec))
+
+
+def stream_window_frames(window_seconds: float, frame_rate: float, max_positions: int) -> int:
+    """W = round(window_seconds * frame_rate) latent frames, checked against 8 <= W <= max_positions."""
+    W = int(round(float(window_seconds) * float(frame_rate)))
+    if not 8 <= W <= int(max_positions):
+        raise ValueError(f"window_seconds={window_seconds} gives W={W} latent frames; a stream window needs "
+                         f"8 <= W <= {int(max_positions)} (the model's position table)")
+    return W
 
 
 def window_rows_budget() -> int:
