@@ -113,6 +113,16 @@ int sab_decode(sab_engine* e, const float* latent, int Bc, int T, float* wav, vo
 int64_t sab_launch_count(sab_engine* e, int reset);
 /* Workspace bytes currently held. */
 int64_t sab_workspace_bytes(sab_engine* e);
+/* Plan residency.  sab_prepare fills the DiT plan of its (B, candidates, T, L), building it if it is not resident, and
+ * sab_solve / sab_dit_forward run the plan the last sab_prepare filled; each plan keeps its own workspace, time tables
+ * and captured solve graph.  At most dit_plans DiT plans and codec_plans_per_direction codec plans per direction
+ * (keyed by (items per chunk, length)) stay resident; the least recently used go first.  The defaults are 1 and 3.
+ * Lowering a limit evicts at once (after a device synchronise).  Both limits must be >= 1. */
+int sab_set_plan_limits(sab_engine* e, int dit_plans, int codec_plans_per_direction);
+/* Counts since sab_create: DiT plans built, solve graphs captured, codec plans built (both directions); and the plans
+ * resident now (codec: both directions).  Any pointer may be NULL. */
+int sab_plan_stats(sab_engine* e, int64_t* dit_plan_builds, int64_t* graph_captures, int64_t* codec_plan_builds,
+                   int* dit_plans_resident, int* codec_plans_resident);
 /* Live per-kernel timing for roofline reporting: with profiling on, one CUDA event is recorded in front of
  * every launch on `stream`; sab_profile_report aggregates the inter-event times per kernel tag as JSON
  * ({"tag": {"launches","ms","flops","bytes"}}) and clears the log. */

@@ -83,7 +83,7 @@ class SabTestGemmDesc(ctypes.Structure):
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
-    "sab_workspace_bytes", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_blend_windows", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_workspace_bytes", "sab_set_plan_limits", "sab_plan_stats", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_blend_windows", "sab_test_aa_taps", "sab_test_solver_grid",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -116,6 +116,9 @@ def lib() -> ctypes.CDLL:
         L.sab_launch_count.restype = i64
         L.sab_workspace_bytes.argtypes = [vp]
         L.sab_workspace_bytes.restype = i64
+        L.sab_set_plan_limits.argtypes = [vp, i32, i32]
+        L.sab_plan_stats.argtypes = [vp, ctypes.POINTER(i64), ctypes.POINTER(i64), ctypes.POINTER(i64),
+                                     ctypes.POINTER(i32), ctypes.POINTER(i32)]
         L.sab_profile.argtypes = [vp, i32, vp]
         L.sab_profile_report.argtypes = [vp, ctypes.c_char_p, i64, vp]
         L.sab_test_gemm.argtypes = [i32, i32, i32, vp, vp, vp, i32, i32, i32, vp]
@@ -284,6 +287,20 @@ class Engine:
 
     def workspace_bytes(self) -> int:
         return int(lib().sab_workspace_bytes(self._h))
+
+    DEFAULT_PLAN_LIMITS = (1, 3)    # include/samaudio_b200.h sab_set_plan_limits
+
+    def set_plan_limits(self, dit_plans: int, codec_plans_per_direction: int):
+        check(lib().sab_set_plan_limits(self._h, int(dit_plans), int(codec_plans_per_direction)))
+
+    def plan_stats(self) -> dict:
+        """Plans built and solve graphs captured since the engine was created, and the plans resident now."""
+        b, g, cb = ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int64()
+        dr, cr = ctypes.c_int(), ctypes.c_int()
+        check(lib().sab_plan_stats(self._h, ctypes.byref(b), ctypes.byref(g), ctypes.byref(cb), ctypes.byref(dr),
+                                   ctypes.byref(cr)))
+        return {"dit_plan_builds": b.value, "graph_captures": g.value, "codec_plan_builds": cb.value,
+                "dit_plans_resident": dr.value, "codec_plans_resident": cr.value}
 
 
 class T5Engine:

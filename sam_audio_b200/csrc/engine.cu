@@ -415,9 +415,14 @@ struct sab_engine {
   std::vector<DecBlockW> dec_blocks;
   float* dec_final_alpha; float *dec_last_w, *dec_last_b;  // Snake + Conv1d(C,1,7) + tanh
 
-  std::unique_ptr<DitPlan> dit;
+  // resident DiT plans, one per (B, candidates, T, L), least recently used evicted beyond max_dit_plans; `dit` is the
+  // one the last sab_prepare filled, which sab_solve / sab_dit_forward run
+  std::vector<std::unique_ptr<DitPlan>> dit_plans;
+  DitPlan* dit = nullptr;
   std::map<std::pair<int, long long>, std::unique_ptr<CodecPlan>> enc_plans, dec_plans;
   int64_t plan_clock = 0;
+  size_t max_dit_plans = 1, max_codec_plans = 3;   // sab_set_plan_limits
+  int64_t dit_plan_builds = 0, graph_captures = 0, codec_plan_builds = 0;   // sab_plan_stats
 
   ~sab_engine();
 };
@@ -728,6 +733,7 @@ struct DitPlan {
   int solve_method = 0;              // SAB_ODE_* of the cached time tables / captured graph
   int64_t time_cap = 0;              // capacity of time_dev (floats)
   float* rk[4] = {nullptr, nullptr, nullptr, nullptr};   // rk4 stage velocities
+  int64_t last_use = 0;              // engine plan_clock of the last sab_prepare that selected this plan
   ~DitPlan() { if (solve_graph) cudaGraphExecDestroy(solve_graph); }
 };
 
@@ -771,7 +777,7 @@ static void build_time_state(sab_engine* e, DitPlan& p, TimeState& ts, int R) {
 // the once-per-call GEMMs and the text path (memory, y_embedder, cross K/V) run on B clips and the per-sequence
 // consumers index clip = sequence / cand.  Inside sab_solve every sequence sees the same time, so the text path of
 // a clip is the same for all of its candidates; sab_dit_forward is only used with cand == 1.
-static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_ids_cap) {
+static std::unique_ptr<DitPlan> build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_ids_cap) {
   const int Bc = B * cand;
   const sab_config& c = e->cfg;
   const int d = c.dim, hid = c.ffn_hidden, NL = c.n_layers;
@@ -937,7 +943,22 @@ static void build_dit_plan(sab_engine* e, int B, int cand, int T, int L, int n_i
     f += p.fold_flops;
   }
   p.flops_per_eval = f;
-  e->dit = std::move(P);
+  e->dit_plan_builds++;
+  return P;
+}
+
+// Drop resident DiT plans, least recently used first, until at most `keep` remain.  A victim's workspace and graph may
+// still be in use by enqueued work on any stream.
+static void evict_dit_plans(sab_engine* e, size_t keep) {
+  if (e->dit_plans.size() <= keep) return;
+  SAB_CUDA(cudaDeviceSynchronize());
+  while (e->dit_plans.size() > keep) {
+    auto victim = e->dit_plans.begin();
+    for (auto it = e->dit_plans.begin(); it != e->dit_plans.end(); ++it)
+      if ((*it)->last_use < (*victim)->last_use) victim = it;
+    if (victim->get() == e->dit) e->dit = nullptr;
+    e->dit_plans.erase(victim);
+  }
 }
 
 // =====================================================================================================
@@ -1240,15 +1261,17 @@ struct CodecPlan {
   int64_t last_use = 0;
 };
 // A few resident plans per direction (ragged traffic alternates between clip lengths / tail chunks): the least
-// recently used one goes when a new shape arrives and kMaxCodecPlans are resident.
-constexpr size_t kMaxCodecPlans = 3;
-static void evict_codec_plans(sab_engine* e, std::map<std::pair<int, long long>, std::unique_ptr<CodecPlan>>& plans) {
-  if (plans.size() < kMaxCodecPlans) return;
+// recently used ones go until at most `keep` are resident (e->max_codec_plans - 1 before a new shape is planned).
+static void evict_codec_plans(sab_engine* e, std::map<std::pair<int, long long>, std::unique_ptr<CodecPlan>>& plans,
+                              size_t keep) {
+  if (plans.size() <= keep) return;
   SAB_CUDA(cudaDeviceSynchronize());          // the victim's workspace may still be in use by enqueued work
-  auto victim = plans.begin();
-  for (auto it = plans.begin(); it != plans.end(); ++it)
-    if (it->second->last_use < victim->second->last_use) victim = it;
-  plans.erase(victim);
+  while (plans.size() > keep) {
+    auto victim = plans.begin();
+    for (auto it = plans.begin(); it != plans.end(); ++it)
+      if (it->second->last_use < victim->second->last_use) victim = it;
+    plans.erase(victim);
+  }
 }
 
 static int pick_bn(int N) {
@@ -1321,7 +1344,8 @@ static CodecPlan* get_enc_plan(sab_engine* e, int items, long long S) {
   auto key = std::make_pair(items, S);
   auto it = e->enc_plans.find(key);
   if (it != e->enc_plans.end()) { it->second->last_use = ++e->plan_clock; return it->second.get(); }
-  evict_codec_plans(e, e->enc_plans);
+  evict_codec_plans(e, e->enc_plans, e->max_codec_plans - 1);
+  e->codec_plan_builds++;
   const sab_config& c = e->cfg;
   auto CP = std::make_unique<CodecPlan>();
   CodecPlan& cp = *CP;
@@ -1392,7 +1416,8 @@ static CodecPlan* get_dec_plan(sab_engine* e, int items, long long T) {
   auto key = std::make_pair(items, T);
   auto it = e->dec_plans.find(key);
   if (it != e->dec_plans.end()) { it->second->last_use = ++e->plan_clock; return it->second.get(); }
-  evict_codec_plans(e, e->dec_plans);
+  evict_codec_plans(e, e->dec_plans, e->max_codec_plans - 1);
+  e->codec_plan_builds++;
   const sab_config& c = e->cfg;
   auto CP = std::make_unique<CodecPlan>();
   CodecPlan& cp = *CP;
@@ -1463,7 +1488,8 @@ static CodecPlan* get_dec_plan(sab_engine* e, int items, long long T) {
 }
 
 sab_engine::~sab_engine() {
-  dit.reset();
+  dit = nullptr;
+  dit_plans.clear();
   enc_plans.clear();
   dec_plans.clear();
   if (staging) cudaFree(staging);
@@ -1572,7 +1598,7 @@ int sab_load_weight(sab_engine* e, const char* name, const float* data, const in
   if (!is_device) SAB_CUDA(cudaStreamSynchronize(st));  // staging buffer is reused by the next call
   s.loaded = true;
   e->finalized = false;
-  if (e->dit) e->dit->ts_solve.valid = false;           // hoisted adaLN tables depend on the weights
+  for (auto& p : e->dit_plans) p->ts_solve.valid = false;   // hoisted adaLN tables depend on the weights
   SAB_API_END
 }
 
@@ -1636,13 +1662,24 @@ int sab_prepare(sab_engine* e, int B, int candidates, int T, int L, const float*
   SAB_CHECK(no_text ? L == 1 : text_features != nullptr, "text_features missing (or SAB_PREP_NO_TEXT with L != 1)");
   SAB_CHECK(no_anchor || (anchor_ids && anchor_alignment && n_ids > 0), "anchor tensors missing");
   cudaStream_t st = (cudaStream_t)stream;
-  if (!e->dit || e->dit->B != B || e->dit->cand != candidates || e->dit->T != T || e->dit->L != L ||
-      n_ids > e->dit->n_ids_cap) {
+  DitPlan* sel = nullptr;
+  for (auto& q : e->dit_plans)
+    if (q->B == B && q->cand == candidates && q->T == T && q->L == L) sel = q.get();
+  if (!sel || n_ids > sel->n_ids_cap) {
     SAB_CUDA(cudaStreamSynchronize(st));
-    e->dit.reset();
-    build_dit_plan(e, B, candidates, T, L, std::max(64, n_ids));   // the anchor-id table grows with the longest id list
+    e->dit = nullptr;                                  // until the new plan exists
+    if (sel) {                                         // too small an anchor-id table: this shape is planned anew
+      sel->last_use = -1;
+      evict_dit_plans(e, e->dit_plans.size() - 1);
+    }
+    evict_dit_plans(e, e->max_dit_plans - 1);
+    // the anchor-id table grows with the longest id list
+    e->dit_plans.push_back(build_dit_plan(e, B, candidates, T, L, std::max(64, n_ids)));
+    sel = e->dit_plans.back().get();
   }
-  DitPlan& p = *e->dit;
+  sel->last_use = ++e->plan_clock;
+  e->dit = sel;
+  DitPlan& p = *sel;
   const sab_config& c = e->cfg;
   const int d = c.dim;
   SAB_CHECK(n_ids <= p.n_ids_cap, "too many anchors per clip (%d > %d)", n_ids, p.n_ids_cap);
@@ -1807,6 +1844,7 @@ int sab_solve(sab_engine* e, const float* noise, int n_steps, int method, float*
     SAB_CUDA(cudaGraphInstantiate(&p.solve_graph, g, 0));
     SAB_CUDA(cudaGraphDestroy(g));
     p.solve_graph_steps = n_steps;
+    e->graph_captures++;
     p.solve_graph_launches = e->launches - launches_before;
     e->launches = launches_before;   // counted when the graph is launched
   }
@@ -2034,10 +2072,33 @@ int64_t sab_launch_count(sab_engine* e, int reset) {
 int64_t sab_workspace_bytes(sab_engine* e) {
   if (!e) return -1;
   int64_t b = e->wpool.bytes;
-  if (e->dit) b += e->dit->pool.bytes;
+  for (auto& p : e->dit_plans) b += p->pool.bytes;
   for (auto& kv : e->enc_plans) b += kv.second->pool.bytes;
   for (auto& kv : e->dec_plans) b += kv.second->pool.bytes;
   return b;
+}
+
+int sab_set_plan_limits(sab_engine* e, int dit_plans, int codec_plans_per_direction) {
+  SAB_API_BEGIN_E(e)
+  SAB_CHECK(dit_plans >= 1 && codec_plans_per_direction >= 1, "plan limits must be >= 1 (got %d, %d)", dit_plans,
+            codec_plans_per_direction);
+  e->max_dit_plans = (size_t)dit_plans;
+  e->max_codec_plans = (size_t)codec_plans_per_direction;
+  evict_dit_plans(e, e->max_dit_plans);
+  evict_codec_plans(e, e->enc_plans, e->max_codec_plans);
+  evict_codec_plans(e, e->dec_plans, e->max_codec_plans);
+  SAB_API_END
+}
+
+int sab_plan_stats(sab_engine* e, int64_t* dit_plan_builds, int64_t* graph_captures, int64_t* codec_plan_builds,
+                   int* dit_plans_resident, int* codec_plans_resident) {
+  SAB_API_BEGIN_E(e)
+  if (dit_plan_builds) *dit_plan_builds = e->dit_plan_builds;
+  if (graph_captures) *graph_captures = e->graph_captures;
+  if (codec_plan_builds) *codec_plan_builds = e->codec_plan_builds;
+  if (dit_plans_resident) *dit_plans_resident = (int)e->dit_plans.size();
+  if (codec_plans_resident) *codec_plans_resident = (int)(e->enc_plans.size() + e->dec_plans.size());
+  SAB_API_END
 }
 
 int sab_profile(sab_engine* e, int enable, void* stream) {

@@ -95,6 +95,7 @@ class SAMAudio(torch.nn.Module):
         self.text_ranker = None         # the contract in sam_audio_b200/ranking.py; selection follows the reference
         self._engine: Optional[_capi.Engine] = None
         self._state: Optional[Dict[str, torch.Tensor]] = None
+        self._plan_limits: Dict[int, Any] = {}          # open stream groups' plan residency (_hold_plan_limits)
         self._device = torch.device("cpu")
         self.register_buffer("_anchor", torch.zeros(1), persistent=False)
 
@@ -367,19 +368,9 @@ class SAMAudio(torch.nn.Module):
         latent = torch.empty(B * c, T, C2, device=dev, dtype=torch.float32)
         return _capi.blend_windows(win_lat, seq.to(dev), start.to(dev), flags.to(dev), window_ramp(Tw), latent)
 
-    def stream(self, description: str, window_seconds: float = 10.0, seed: int = 0,
-               ode_opt: Dict[str, Any] = DFLT_ODE_OPT, reranking_candidates: int = 1, anchors=None,
-               masked_video=None):
-        """Separation of audio that arrives in chunks (sam_audio_b200.stream, DESIGN.md section 3):
-
-            s = model.stream(description="man speaking")
-            for chunk in source:          # [S] or [1, S] float samples at the model's rate, any S >= 1
-                out = s.push(chunk)       # out.target / out.residual: the samples that became final
-            tail = s.flush()              # the rest; the stream is closed afterwards
-
-        The stream is solved as windows of W = round(window_seconds * 25) latent frames, 8 <= W <= max_positions; the
-        default 10 s keeps the DiT on its short-sequence attention (T <= 256).  Text prompts with one candidate only."""
-        from .stream import SeparationStream
+    def _stream_args(self, window_seconds: float, ode_opt: Dict[str, Any], reranking_candidates: int, anchors,
+                     masked_video):
+        """(W, n_steps, method) of a stream, after the checks stream() and stream_group() share."""
         from .windows import stream_window_frames
         cc = self.cfg.audio_codec
         W = stream_window_frames(window_seconds, cc.sample_rate / cc.hop_length, self.cfg.transformer.max_positions)
@@ -392,10 +383,64 @@ class SAMAudio(torch.nn.Module):
         if masked_video is not None:
             raise NotImplementedError("a stream takes no masked video: video frames would need a time base aligned with "
                                       "the stream, which it does not have yet")
+        n_steps, method = _ode_grid(ode_opt)
+        return W, n_steps, method
+
+    def stream(self, description: str, window_seconds: float = 10.0, seed: int = 0,
+               ode_opt: Dict[str, Any] = DFLT_ODE_OPT, reranking_candidates: int = 1, anchors=None,
+               masked_video=None):
+        """Separation of audio that arrives in chunks (sam_audio_b200.stream, DESIGN.md section 3):
+
+            s = model.stream(description="man speaking")
+            for chunk in source:          # [S] or [1, S] float samples at the model's rate, any S >= 1
+                out = s.push(chunk)       # out.target / out.residual: the samples that became final
+            tail = s.flush()              # the rest; the stream is closed afterwards
+
+        The stream is solved as windows of W = round(window_seconds * 25) latent frames, 8 <= W <= max_positions; the
+        default 10 s keeps the DiT on its short-sequence attention (T <= 256).  Text prompts with one candidate only.
+        The stream is the one stream of a group of its own (stream_group) that keeps the engine's default plan
+        residency."""
+        from .stream import StreamGroup
+        W, n_steps, method = self._stream_args(window_seconds, ode_opt, reranking_candidates, anchors, masked_video)
         if not isinstance(description, str):
             raise TypeError("a stream separates one source: description must be one string")
-        n_steps, method = _ode_grid(ode_opt)
-        return SeparationStream(self, description, W, int(seed), n_steps, method)
+        return StreamGroup(self, W, n_steps, method, resident_plans=False).open(description, seed=int(seed))
+
+    def stream_group(self, window_seconds: float = 10.0, ode_opt: Dict[str, Any] = DFLT_ODE_OPT,
+                     reranking_candidates: int = 1, anchors=None, masked_video=None):
+        """Many live streams advanced together (sam_audio_b200.stream, DESIGN.md section 3):
+
+            group = model.stream_group(window_seconds=10.0)
+            a = group.open("man speaking", seed=0)      # a stream, with push / flush as from stream()
+            b = group.open("dog barking", seed=7)
+            outs = group.push({a: chunk_a, b: chunk_b})  # one tick -> {stream: StreamOutput}
+            tails = group.flush([a, b])                  # ends and closes them (a.flush() alone works too)
+            group.close()                                # flushes what is still open; also on leaving a `with` block
+
+        Every stream of a group has the same W and ODE grid; prompts and seeds are per stream, and streams may open and
+        close at any tick.  A tick solves every window that becomes ready in it, from all its streams, in one batched
+        solve, and each stream's output is bit-identical to what stream() returns for the same pushes, whatever the other
+        streams do, as long as every prompt of the group has at most 8 tokens (a longer one moves the whole group to the
+        unfused cross-attention, whose bits depend on the padded text length).  While the group is open the engine keeps
+        one DiT plan per bucket of window counts it has used resident (and the codec plans of those buckets), so ticks
+        of varying size do not re-plan; close() restores the default residency, and so does collecting a group dropped
+        without close().  A flush tick reuses the buckets of earlier ticks, so ending many streams at once plans no
+        larger DiT bucket beside them."""
+        from .stream import StreamGroup
+        W, n_steps, method = self._stream_args(window_seconds, ode_opt, reranking_candidates, anchors, masked_video)
+        return StreamGroup(self, W, n_steps, method, resident_plans=True)
+
+    def _hold_plan_limits(self, holder, limits) -> None:
+        """Engine plan residency: the largest (DiT plans, codec plans per direction) any open stream group holds, the
+        engine's defaults when none does.  `holder` is a group's key object; limits=None releases its hold."""
+        if limits is None:
+            self._plan_limits.pop(id(holder), None)
+        else:
+            self._plan_limits[id(holder)] = limits
+        if self._engine is None:
+            return
+        held = [_capi.Engine.DEFAULT_PLAN_LIMITS] + list(self._plan_limits.values())
+        self._engine.set_plan_limits(max(h[0] for h in held), max(h[1] for h in held))
 
     def predict_spans(self, batch: Batch, audio_features: torch.Tensor, audio_pad_mask: torch.Tensor) -> Batch:
         """Reference model.py:231-245: frame-level span predictor on the first 128 latent channels -> "+" anchors ->

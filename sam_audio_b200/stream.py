@@ -1,33 +1,45 @@
-"""Streaming separation: ``SAMAudio.stream()`` separates audio pushed in chunks (DESIGN.md section 3).
+"""Streaming separation: ``SAMAudio.stream()`` and ``SAMAudio.stream_group()`` separate audio pushed in chunks
+(DESIGN.md section 3).
 
 A stream is solved as windows of W latent frames that start every H = W - W // 8 frames (sam_audio_b200.windows), on
-the same library calls as ``separate()``:
+the same library calls as ``separate()``.  Streams live in a ``StreamGroup`` (``SAMAudio.stream()`` is a group of one),
+and a tick of the group advances the streams it is given with one batched call per step:
 
 - encode: the frames a window adds are encoded from their samples plus the encoder's halo on each side
   (``sab_codec_tiling``); the first slice starts at sample 0 and the last ends at the stream's end, where the codec's
-  zero fill is the clip edge as in an un-tiled encode, so the features equal those of the whole recording;
-- solve: each window is prepared and solved as a clip of W frames with the stream's text; windows made ready by one
-  push are solved as one group;
-- blend: the frames that became final are cross-faded from the last two solved windows by ``sab_blend_windows`` into
-  an output of just those frames (window starts relative to the first of them);
-- decode: final frames are decoded with the decoder's halo of final frames on each side, and only the middle is kept.
+  zero fill is the clip edge as in an un-tiled encode, so the features equal those of the whole recording.  Slices of
+  equal length, from any stream, are the items of one ``sab_encode``;
+- solve: every window that becomes ready in the tick is prepared and solved as a clip of W frames with its stream's
+  text (padded to the group's token count), all of them in one ``sab_prepare`` + ``sab_solve`` per group of
+  ``window_groups``;
+- blend: the frames that became final are cross-faded from each stream's last solved windows by ``sab_blend_windows``
+  into an output of just those frames (window starts relative to the first of them), one output sequence per stream;
+- decode: final frames are decoded with the decoder's halo of final frames on each side, and only the middle is kept;
+  slices of equal length are the items of one ``sab_decode``.
+
+Each planned call runs at an item count rounded up to a bucket (``windows.stream_bucket``), the spare slots repeating a
+live item, so the engine keeps one resident plan per bucket.  An item's result does not depend on the other items of
+its call, so a stream's output is bit-identical whatever the other streams of its group do.
 
 The noise of frame t is row t % H of block t // H, drawn from a generator seeded by (seed, block): overlapping windows
 start from the same noise rows, and nothing depends on how the input was chunked.  Device memory stays bounded by the
 window length, whatever the stream's length: two windows of latents, about W plus two halos of samples and features,
-and the engine's cached plans.  PyTorch only allocates, slices and concatenates here; the arithmetic runs in
+and the engine's resident plans.  PyTorch only allocates, slices and concatenates here; the arithmetic runs in
 libsamaudio_b200.so.
 """
 from __future__ import annotations
 
+import weakref
+from collections import defaultdict
 from dataclasses import dataclass
-from typing import List
+from typing import Dict, Iterable, List, Mapping
 
 import torch
 
 from . import _capi
-from .windows import (stream_emit_end, stream_final_frames, stream_frames_available, stream_hop,
-                      stream_window_starts, stream_windows_ready, window_groups, window_ramp, window_rows_budget)
+from .windows import (stream_bucket, stream_emit_end, stream_final_frames, stream_flush_rows,
+                      stream_frames_available, stream_group_capacity, stream_hop, stream_tick_groups, stream_window_starts,
+                      stream_windows_ready, window_ramp, window_rows_budget)
 
 _NULL_ANCHOR_IDS = (0, 3)   # the processor's ids of a clip without anchors: <null>, <pad> (processor.py)
 
@@ -59,33 +71,50 @@ def stream_noise(seed: int, f0: int, f1: int, block: int, channels: int = 256, d
     return torch.cat(rows)[f0 - b0 * block:f1 - b0 * block]
 
 
-class SeparationStream:
-    """Returned by ``SAMAudio.stream()``; see there.  ``push`` returns the samples that became final, ``flush`` the
-    rest, and the concatenation of everything returned is ceil(n / hop) * hop samples for n samples pushed."""
+def check_tick(group, streams: List) -> None:
+    """The streams of one tick must be distinct open streams of this group (and so share its window length)."""
+    seen = set()
+    for s in streams:
+        if getattr(s, "group", None) is not group:
+            raise ValueError("a tick takes the group's own streams: this stream belongs to another group")
+        if s.closed:
+            raise RuntimeError("the stream is closed: flush() has been called")
+        if s.W != group.W:
+            raise ValueError(f"stream window of {s.W} frames in a group of {group.W}-frame windows")
+        if id(s) in seen:
+            raise ValueError("a stream appears twice in one tick")
+        seen.add(id(s))
 
-    def __init__(self, model, description: str, W: int, seed: int, n_steps: int, method: str):
-        self.model = model
-        eng = model._ensure_engine()
-        cc = model.cfg.audio_codec
-        self.W, self.O, self.H = W, window_ramp(W), stream_hop(W)
-        self.hop = cc.hop_length
-        self.C = 2 * cc.codebook_dim
-        self.seed, self.n_steps, self.method = seed, n_steps, method
-        self.device = model._device
-        self.halo_enc, _ = eng.codec_tiling(False, W)
-        self.halo_dec, _ = eng.codec_tiling(True, W)
-        # with an encoder halo, no window before flush() reaches the last frame, so flush() always solves the window
-        # that carries the stream's end (WIN_LAST)
-        assert self.halo_enc >= 1
+
+def _samples(chunk: torch.Tensor) -> torch.Tensor:
+    if chunk.dim() == 2 and chunk.shape[0] == 1:
+        chunk = chunk[0]
+    if chunk.dim() != 1 or chunk.numel() < 1:
+        raise ValueError(f"push() takes [S] or [1, S] samples with S >= 1, got shape {tuple(chunk.shape)}")
+    return chunk
+
+
+class SeparationStream:
+    """Returned by ``SAMAudio.stream()`` and ``StreamGroup.open()``; see there.  ``push`` returns the samples that became
+    final, ``flush`` the rest, and the concatenation of everything returned is ceil(n / hop) * hop samples for n samples
+    pushed.  ``push`` and ``flush`` are ticks of the stream's group with this stream alone."""
+
+    def __init__(self, group: "StreamGroup", description: str, seed: int):
+        self.group = group
+        self.model = group.model
+        self.W, self.O, self.H, self.hop, self.C = group.W, group.O, group.H, group.hop, group.C
+        self.seed = seed
+        self.device = group.device
         with torch.cuda.device(self.device):
-            tf, tm = model.text_encoder([description])          # encoded once for the whole stream
+            tf, tm = self.model.text_encoder([description])     # encoded once for the whole stream
         self._text = tf.to(self.device, torch.float32).contiguous()
         self._text_mask = tm.to(self.device).contiguous()
-        self._ids = torch.tensor([_NULL_ANCHOR_IDS], dtype=torch.long, device=self.device)
+        self.n_tokens = self._text.shape[1]
         # samples [wav0, n) live in _buf[:n - wav0]; _spare has the same size and takes the kept samples on a trim
         self._buf = self._spare = None
         self._wav0 = 0
         self.n_samples = 0
+        self.n_final = None                                    # frames of the stream, known at flush()
         self._enc_end = 0                                      # frames [0, _enc_end) are encoded ...
         self._feat0 = 0                                        # ... and [_feat0, _enc_end) are kept in _feat
         self._feat = torch.empty(0, self.C, device=self.device)
@@ -98,48 +127,23 @@ class SeparationStream:
         self.closed = False
 
     # ------------------------------------------------------------------ public
-    @torch.inference_mode()
     def push(self, chunk: torch.Tensor) -> StreamOutput:
         """Append samples ([S] or [1, S], S >= 1) and return the samples that became final."""
-        self._check_open()
-        if chunk.dim() == 2 and chunk.shape[0] == 1:
-            chunk = chunk[0]
-        if chunk.dim() != 1 or chunk.numel() < 1:
-            raise ValueError(f"push() takes [S] or [1, S] samples with S >= 1, got shape {tuple(chunk.shape)}")
-        x = chunk.to(device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            self._append(x)
-            avail = stream_frames_available(self.n_samples, self.hop, self.halo_enc)
-            k1 = stream_windows_ready(avail, self.W)
-            return self._advance(k1, flushed=False)
+        return self.group.push({self: chunk})[self]
 
-    @torch.inference_mode()
     def flush(self) -> StreamOutput:
         """End the stream: solve the windows that cover the rest (the last padded past the end as in a padded batch),
         return every sample not returned yet, and close the stream."""
-        self._check_open()
-        self.closed = True
-        with torch.cuda.device(self.device):
-            if self.n_samples == 0:
-                return self._output([])
-            T = -(-self.n_samples // self.hop)
-            self.n_final = T
-            out = self._advance(len(stream_window_starts(T, self.W)), flushed=True)
-        self._buf = self._spare = self._feat = self._lat = self._prev = None
-        return out
+        return self.group.flush([self])[self]
 
     def workspace_bytes(self) -> int:
         return self.model._ensure_engine().workspace_bytes()
 
-    # ------------------------------------------------------------------ steps
-    def _check_open(self):
-        if self.closed:
-            raise RuntimeError("the stream is closed: flush() has been called")
-
+    # ------------------------------------------------------------------ state
     def _append(self, x: torch.Tensor):
         held, S = self.n_samples - self._wav0, x.numel()
         if self._buf is None or held + S > self._buf.numel():
-            cap = max(held + S, (self.W + 2 * self.halo_enc) * self.hop + S)
+            cap = max(held + S, (self.W + 2 * self.group.halo_enc) * self.hop + S)
             buf = torch.empty(cap, device=self.device, dtype=torch.float32)
             if held:
                 buf[:held].copy_(self._buf[:held])
@@ -149,7 +153,7 @@ class SeparationStream:
 
     def _trim_samples(self):
         """Drop the samples no later encode reads: the next one starts halo_enc frames before _enc_end."""
-        keep0 = max(0, self._enc_end - self.halo_enc) * self.hop
+        keep0 = max(0, self._enc_end - self.group.halo_enc) * self.hop
         if keep0 <= self._wav0:
             return
         a, b = keep0 - self._wav0, self.n_samples - self._wav0
@@ -157,109 +161,18 @@ class SeparationStream:
         self._buf, self._spare = self._spare, self._buf
         self._wav0 = keep0
 
-    def _encode(self, f1: int, flushed: bool):
-        """Encode frames [_enc_end, f1) into _feat.  The encoder reads halo_enc frames of samples on each side; at the
-        stream's start the slice starts at sample 0, at flush() it ends at the (reflect-padded) end of the stream."""
-        a = self._enc_end
-        if f1 <= a:
-            return
-        s0 = max(0, a - self.halo_enc)
-        if flushed:
-            wav = self.model._pad(self._buf[s0 * self.hop - self._wav0:self.n_samples - self._wav0].view(1, -1))
-            s1 = f1
-        else:
-            s1 = f1 + self.halo_enc
-            wav = self._buf[s0 * self.hop - self._wav0:s1 * self.hop - self._wav0].view(1, -1)
-        assert wav.shape[1] == (s1 - s0) * self.hop
-        feats = torch.empty(1, s1 - s0, self.C, device=self.device, dtype=torch.float32)
-        self.model._ensure_engine().encode(wav.contiguous(), feats)
-        self._feat = torch.cat([self._feat, feats[0, a - s0:f1 - s0]])
-        self._enc_end = f1
+    def _text_at(self, L: int):
+        """Text features and mask padded to L tokens (zero features, masked)."""
+        n = self.n_tokens
+        if n == L:
+            return self._text[0], self._text_mask[0]
+        f = torch.zeros(L, self._text.shape[2], device=self.device, dtype=torch.float32)
+        m = torch.zeros(L, dtype=self._text_mask.dtype, device=self.device)
+        f[:n], m[:n] = self._text[0], self._text_mask[0]
+        return f, m
 
-    def _advance(self, k_end: int, flushed: bool) -> StreamOutput:
-        """Solve windows [windows_solved, k_end) group by group, blending and decoding what each group makes final."""
-        W, H = self.W, self.H
-        pieces: List[torch.Tensor] = []
-        k0 = self.windows_solved
-        groups = window_groups(k_end - k0, 1, W, window_rows_budget())
-        for g0, g1 in groups:
-            ka, kb = k0 + g0, k0 + g1
-            if flushed:
-                self._encode(self.n_final, True)
-            else:
-                for k in range(ka, kb):                        # one fixed-shape encode per window
-                    self._encode(k * H + W, False)
-            self._solve(ka, kb, flushed and kb == k_end, k_end)
-            pieces.append(self._decode(flushed and kb == k_end))
-        if not flushed:
-            self._trim_samples()
-        return self._output(pieces)
-
-    def _solve(self, ka: int, kb: int, last_group: bool, k_end: int):
-        """Prepare and solve windows [ka, kb) as one batch of clips of W frames, then blend the frames they make final
-        from them and the previously solved window."""
-        eng = self.model._ensure_engine()
-        W, H, C, dev = self.W, self.H, self.C, self.device
-        g = kb - ka
-        n_valid = self.n_final if last_group else None
-        need = (kb - 1) * H + W                                # features of frames [ka * H, need)
-        if need > self._enc_end:                               # past the end of the stream: zero, under the pad mask
-            self._feat = torch.cat([self._feat, torch.zeros(need - self._enc_end, C, device=dev)])
-            self._enc_end = need
-        f = self._feat
-        feats = torch.stack([f[k * H - self._feat0:k * H - self._feat0 + W] for k in range(ka, kb)])
-        pad = torch.ones(g, W, dtype=torch.bool, device=dev)
-        align = torch.zeros(g, W, dtype=torch.long, device=dev)
-        if n_valid is not None:
-            for i, k in enumerate(range(ka, kb)):
-                v = max(0, n_valid - k * H)
-                pad[i, v:] = False
-                align[i, v:] = 1                               # the processor's <pad> alignment for pad frames
-        self.model._install_conditioning(feats, self._text.expand(g, -1, -1), self._text_mask.expand(g, -1), None,
-                                         self._ids.expand(g, -1), align, pad, candidates=1)
-        n_prev = 0 if self._prev is None else 1
-        win = torch.empty(n_prev + g, W, C, device=dev, dtype=torch.float32)
-        if n_prev:
-            win[0].copy_(self._prev)
-        for i, k in enumerate(range(ka, kb)):
-            win[n_prev + i].copy_(stream_noise(self.seed, k * H, k * H + W, H, C, dev))
-        rows = win[n_prev:]
-        eng.solve(rows, self.n_steps, rows, self.method)
-        self.windows_solved = kb
-        # blend the frames that became final; starts are relative to the first of them
-        f_old = self.final_frames
-        f_new = stream_final_frames(kb, W, self.n_final if last_group else -1)
-        ks = list(range(ka - n_prev, kb))
-        seq = torch.zeros(len(ks), dtype=torch.int32, device=dev)
-        start = torch.tensor([k * H - f_old for k in ks], dtype=torch.int32, device=dev)
-        flags = torch.tensor([_capi.WIN_FIRST * (k == 0) + _capi.WIN_LAST * (last_group and k == k_end - 1) for k in ks],
-                             dtype=torch.uint8, device=dev)
-        out = torch.empty(1, f_new - f_old, C, device=dev, dtype=torch.float32)
-        _capi.blend_windows(win, seq, start, flags, self.O, out)
-        self._lat = torch.cat([self._lat, out[0]])
-        self.final_frames = f_new
-        self._prev = win[-1]
-        # the next window reads features from frame kb * H on
-        drop = min(kb * H, self._enc_end) - self._feat0
-        self._feat = self._feat[drop:].clone()
-        self._feat0 += drop
-
-    def _decode(self, flushed: bool) -> torch.Tensor:
-        """Decode frames [emitted_frames, emit_end) from the final latent with halo_dec frames on each side; returns
-        [2, samples] (target, residual)."""
-        a, F = self.emitted_frames, self.final_frames
-        b = stream_emit_end(F, self.halo_dec, flushed)
-        if b <= a:
-            return torch.empty(2, 0, device=self.device)
-        d0, d1 = max(0, a - self.halo_dec), F if flushed else b + self.halo_dec
-        lat = self._lat[d0 - self._lat0:d1 - self._lat0].unsqueeze(0).contiguous()
-        wav = torch.empty(1, 2, (d1 - d0) * self.hop, device=self.device, dtype=torch.float32)
-        self.model._ensure_engine().decode(lat, 1, d1 - d0, wav)
-        self.emitted_frames = b
-        keep0 = max(0, b - self.halo_dec)                        # the next decode reads from here on
-        self._lat = self._lat[keep0 - self._lat0:].clone()
-        self._lat0 = keep0
-        return wav[0, :, (a - d0) * self.hop:(b - d0) * self.hop]
+    def _release(self):
+        self._buf = self._spare = self._feat = self._lat = self._prev = None
 
     def _output(self, pieces: List[torch.Tensor]) -> StreamOutput:
         if not pieces:
@@ -267,3 +180,288 @@ class SeparationStream:
             return StreamOutput(target=e, residual=e.clone())
         w = pieces[0] if len(pieces) == 1 else torch.cat(pieces, 1)
         return StreamOutput(target=w[0], residual=w[1])
+
+
+class StreamGroup:
+    """Returned by ``SAMAudio.stream_group()``; see there.  Streams of one group share the window length and the ODE
+    grid; a tick (``push`` / ``flush``) advances any subset of the open streams with batched library calls."""
+
+    def __init__(self, model, W: int, n_steps: int, method: str, resident_plans: bool):
+        self.model = model
+        eng = model._ensure_engine()
+        cc = model.cfg.audio_codec
+        self.W, self.O, self.H = W, window_ramp(W), stream_hop(W)
+        self.hop = cc.hop_length
+        self.C = 2 * cc.codebook_dim
+        self.n_steps, self.method = n_steps, method
+        self.device = model._device
+        self.halo_enc, _ = eng.codec_tiling(False, W)
+        self.halo_dec, _ = eng.codec_tiling(True, W)
+        # with an encoder halo, no window before flush() reaches the last frame, so flush() always solves the window
+        # that carries the stream's end (WIN_LAST)
+        assert self.halo_enc >= 1
+        self.capacity = stream_group_capacity(W, window_rows_budget())
+        self.L = 0                      # text tokens of every window: the longest prompt opened in the group so far
+        self.streams: List[SeparationStream] = []
+        self._ids = torch.tensor([_NULL_ANCHOR_IDS], dtype=torch.long, device=self.device)
+        self.closed = False
+        self._holds_limits = resident_plans
+        self._buckets_used = set()     # item counts of the planned calls of push ticks (the residency follows them)
+        self._solve_buckets = set()    # ... of their solves: the DiT plans a flush tick reuses
+        if resident_plans:
+            # a group dropped without close() gives the residency back when it is collected
+            self._limits_key = object()
+            self._finalizer = weakref.finalize(self, model._hold_plan_limits, self._limits_key, None)
+            self._finalizer.atexit = False
+
+    # ------------------------------------------------------------------ public
+    def open(self, description: str, seed: int = 0) -> SeparationStream:
+        """A new stream of the group with its own prompt and noise seed."""
+        if self.closed:
+            raise RuntimeError("the stream group is closed")
+        if not isinstance(description, str):
+            raise TypeError("a stream separates one source: description must be one string")
+        s = SeparationStream(self, description, int(seed))
+        self.L = max(self.L, s.n_tokens)
+        self.streams.append(s)
+        return s
+
+    @torch.inference_mode()
+    def push(self, chunks: Mapping[SeparationStream, torch.Tensor]) -> Dict[SeparationStream, StreamOutput]:
+        """One tick: append each stream's samples ([S] or [1, S], S >= 1) and return, per stream, the samples that
+        became final."""
+        streams = list(chunks)
+        check_tick(self, streams)
+        xs = [_samples(chunks[s]).to(device=self.device, dtype=torch.float32) for s in streams]
+        with torch.cuda.device(self.device):
+            due = []
+            for s, x in zip(streams, xs):
+                s._append(x)
+                avail = stream_frames_available(s.n_samples, self.hop, self.halo_enc)
+                due.append((s, s.windows_solved, stream_windows_ready(avail, self.W)))
+            out = self._tick(due, flushed=False)
+            for s in streams:
+                s._trim_samples()
+        return out
+
+    @torch.inference_mode()
+    def flush(self, streams: Iterable[SeparationStream]) -> Dict[SeparationStream, StreamOutput]:
+        """One tick that ends the given streams: each returns every sample not returned yet and is closed."""
+        streams = list(streams)
+        check_tick(self, streams)
+        live = [s for s in streams if s.n_samples > 0]
+        try:
+            with torch.cuda.device(self.device):
+                for s in live:
+                    s.n_final = -(-s.n_samples // self.hop)
+                out = self._tick([(s, s.windows_solved, len(stream_window_starts(s.n_final, self.W))) for s in live],
+                                 flushed=True)
+                for s in streams:
+                    out.setdefault(s, s._output([]))
+        finally:
+            # a stream is ended whether or not its last tick succeeded: a failed flush leaves no half-advanced stream
+            # in the group, so close() still works and gives the engine back its residency
+            for s in streams:
+                s.closed = True
+                s._release()
+                self.streams.remove(s)
+        return out
+
+    def close(self) -> Dict[SeparationStream, StreamOutput]:
+        """Flush every open stream, close the group and give the engine back its default plan residency."""
+        self.closed = True
+        try:
+            return self.flush(list(self.streams)) if self.streams else {}
+        finally:
+            self._release_limits()
+
+    def _release_limits(self):
+        if self._holds_limits:
+            self._holds_limits = False
+            self._finalizer.detach()
+            self.model._hold_plan_limits(self._limits_key, None)
+
+    def _slots(self, n: int, flushed: bool, solve: bool) -> List[int]:
+        """stream_bucket of n items.  A push tick may use a new bucket, and the engine's plan residency is raised to
+        the buckets this group has used: one DiT plan per bucket, and per direction two codec slice lengths per bucket
+        (a stream's first window and the later ones) plus one for the varying lengths of flushes, which therefore
+        replace each other.  A flush tick's solve reuses a bucket already used when one is large enough; its encode and
+        decode slices have lengths of their own, so no resident plan fits them and they use no bucket slot."""
+        if not self._holds_limits or (flushed and not solve):
+            return stream_bucket(n, self.capacity)
+        slots = stream_bucket(n, self.capacity, self._solve_buckets if flushed else ())
+        self._solve_buckets.add(len(slots))
+        if len(slots) not in self._buckets_used:
+            self._buckets_used.add(len(slots))
+            k = len(self._buckets_used)
+            self.model._hold_plan_limits(self._limits_key, (k, 2 * k + 1))
+        return slots
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    # ------------------------------------------------------------------ the tick
+    def _tick(self, due, flushed: bool) -> Dict[SeparationStream, StreamOutput]:
+        """Solve windows [k0, k_end) of every (stream, k0, k_end) in due, group by group: encode, solve, blend and decode
+        what each group makes final."""
+        pieces: Dict[SeparationStream, List[torch.Tensor]] = {s: [] for s, _, _ in due}
+        budget = window_rows_budget()
+        if flushed and self._holds_limits:
+            budget = stream_flush_rows(budget, self.W, self._solve_buckets)
+        for grp in stream_tick_groups(due, self.W, budget):
+            self._encode(grp, flushed)
+            rows = self._solve(grp, flushed)
+            self._blend(grp, rows, flushed)
+            for s, piece in self._decode(grp, flushed):
+                pieces[s].append(piece)
+        return {s: s._output(p) for s, p in pieces.items()}
+
+    def _encode(self, grp, flushed: bool):
+        """Encode the frames the group's windows need: [_enc_end, k * H + W) per window, or up to the stream's end at
+        flush().  A slice reads halo_enc frames of samples on each side; at a stream's start it starts at sample 0, at
+        flush() it ends at the (reflect-padded) end of the stream."""
+        hop, halo = self.hop, self.halo_enc
+        jobs = []                                              # (stream, samples, first kept row, end row, new end)
+        for w in grp:
+            s = w.key
+            a = s._enc_end
+            for f1 in ([s.n_final] if flushed else [k * self.H + self.W for k in range(w.ka, w.kb)]):
+                if f1 <= a:
+                    continue
+                s0 = max(0, a - halo)
+                if flushed:
+                    wav = self.model._pad(s._buf[s0 * hop - s._wav0:s.n_samples - s._wav0].view(1, -1))[0]
+                    s1 = f1
+                else:
+                    s1 = f1 + halo
+                    wav = s._buf[s0 * hop - s._wav0:s1 * hop - s._wav0]
+                assert wav.numel() == (s1 - s0) * hop
+                jobs.append((s, wav, a - s0, f1 - s0, f1))
+                a = f1
+        feats = [None] * len(jobs)
+        by_len = defaultdict(list)
+        for i, j in enumerate(jobs):
+            by_len[j[1].numel()].append(i)
+        eng = self.model._ensure_engine()
+        for n, idx in by_len.items():
+            slots = self._slots(len(idx), flushed, solve=False)
+            wav = torch.stack([jobs[idx[i]][1] for i in slots])
+            out = torch.empty(len(slots), n // hop, self.C, device=self.device, dtype=torch.float32)
+            eng.encode(wav, out)
+            for i, ji in enumerate(idx):
+                feats[ji] = out[i]
+        for (s, _, r0, r1, f1), f in zip(jobs, feats):          # in job order: a stream's slices follow each other
+            s._feat = torch.cat([s._feat, f[r0:r1]])
+            s._enc_end = f1
+
+    def _solve(self, grp, flushed: bool) -> torch.Tensor:
+        """Prepare and solve the group's windows as one batch of clips of W frames; returns their latents [n, W, C]."""
+        W, H, C, dev = self.W, self.H, self.C, self.device
+        feats, texts, masks, pads, aligns, noise = [], [], [], [], [], []
+        for w in grp:
+            s = w.key
+            n_valid = s.n_final if flushed and w.last else None
+            need = (w.kb - 1) * H + W                          # features of frames [ka * H, need)
+            if need > s._enc_end:                              # past the end of the stream: zero, under the pad mask
+                s._feat = torch.cat([s._feat, torch.zeros(need - s._enc_end, C, device=dev)])
+                s._enc_end = need
+            tf, tm = s._text_at(self.L)
+            for k in range(w.ka, w.kb):
+                feats.append(s._feat[k * H - s._feat0:k * H - s._feat0 + W])
+                texts.append(tf)
+                masks.append(tm)
+                pad = torch.ones(W, dtype=torch.bool, device=dev)
+                align = torch.zeros(W, dtype=torch.long, device=dev)
+                if n_valid is not None:
+                    v = max(0, n_valid - k * H)
+                    pad[v:] = False
+                    align[v:] = 1                              # the processor's <pad> alignment for pad frames
+                pads.append(pad)
+                aligns.append(align)
+                noise.append(stream_noise(s.seed, k * H, k * H + W, H, C, dev))
+        n = len(feats)
+        slots = self._slots(n, flushed, solve=True)
+        pick = lambda xs: torch.stack([xs[i] for i in slots])   # noqa: E731
+        nb = len(slots)
+        self.model._install_conditioning(pick(feats), pick(texts), pick(masks), None, self._ids.expand(nb, -1),
+                                         pick(aligns), pick(pads), candidates=1)
+        rows = pick(noise)
+        self.model._ensure_engine().solve(rows, self.n_steps, rows, self.method)
+        return rows[:n]
+
+    def _blend(self, grp, rows: torch.Tensor, flushed: bool):
+        """Blend each stream's frames that became final from its previous window and the windows just solved; streams
+        that finalise the same number of frames share one sab_blend_windows call (one output sequence each)."""
+        W, H, C, dev = self.W, self.H, self.C, self.device
+        by_count = defaultdict(list)
+        i = 0
+        for w in grp:
+            s = w.key
+            f_new = stream_final_frames(w.kb, W, s.n_final if flushed and w.last else -1)
+            by_count[f_new - s.final_frames].append((w, rows[i:i + w.kb - w.ka], f_new))
+            i += w.kb - w.ka
+        for count, members in by_count.items():
+            wins, seq, start, flags = [], [], [], []
+            for q, (w, solved, _) in enumerate(members):
+                s = w.key
+                last_group = flushed and w.last
+                ks = list(range(w.ka - (s._prev is not None), w.kb))
+                if s._prev is not None:
+                    wins.append(s._prev[None])
+                wins.append(solved)
+                seq += [q] * len(ks)
+                start += [k * H - s.final_frames for k in ks]
+                flags += [_capi.WIN_FIRST * (k == 0) + _capi.WIN_LAST * (last_group and k == w.kb - 1) for k in ks]
+            win = torch.cat(wins).contiguous()
+            out = torch.empty(len(members), count, C, device=dev, dtype=torch.float32)
+            _capi.blend_windows(win, torch.tensor(seq, dtype=torch.int32, device=dev),
+                                torch.tensor(start, dtype=torch.int32, device=dev),
+                                torch.tensor(flags, dtype=torch.uint8, device=dev), self.O, out)
+            for q, (w, solved, f_new) in enumerate(members):
+                s = w.key
+                s._lat = torch.cat([s._lat, out[q]])
+                s.final_frames = f_new
+                s.windows_solved = w.kb
+                s._prev = solved[-1].clone()
+                # the next window reads features from frame kb * H on
+                drop = min(w.kb * H, s._enc_end) - s._feat0
+                s._feat = s._feat[drop:].clone()
+                s._feat0 += drop
+
+    def _decode(self, grp, flushed: bool):
+        """Decode frames [emitted_frames, emit_end) of each stream of the group from its final latent with halo_dec
+        frames on each side; slices of equal length share one sab_decode.  Yields (stream, [2, samples])."""
+        hop, halo = self.hop, self.halo_dec
+        jobs = []
+        for w in grp:
+            s = w.key
+            a, F = s.emitted_frames, s.final_frames
+            fl = flushed and w.last
+            b = stream_emit_end(F, halo, fl)
+            if b <= a:
+                jobs.append((s, None, 0, 0))
+                continue
+            d0, d1 = max(0, a - halo), F if fl else b + halo
+            jobs.append((s, s._lat[d0 - s._lat0:d1 - s._lat0], (a - d0) * hop, (b - d0) * hop))
+            s.emitted_frames = b
+            keep0 = max(0, b - halo)                               # the next decode reads from here on
+            s._lat = s._lat[keep0 - s._lat0:].clone()
+            s._lat0 = keep0
+        wavs = [None] * len(jobs)
+        by_len = defaultdict(list)
+        for i, j in enumerate(jobs):
+            if j[1] is not None:
+                by_len[j[1].shape[0]].append(i)
+        eng = self.model._ensure_engine()
+        for T, idx in by_len.items():
+            slots = self._slots(len(idx), flushed, solve=False)
+            lat = torch.stack([jobs[idx[i]][1] for i in slots])
+            out = torch.empty(len(slots), 2, T * hop, device=self.device, dtype=torch.float32)
+            eng.decode(lat, len(slots), T, out)
+            for i, ji in enumerate(idx):
+                wavs[ji] = out[i]
+        for (s, _, a, b), wav in zip(jobs, wavs):
+            yield s, (torch.empty(2, 0, device=self.device) if wav is None else wav[:, a:b])

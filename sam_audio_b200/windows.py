@@ -115,3 +115,67 @@ def window_groups(n_windows: int, candidates: int, Tw: int, budget_rows: int) ->
     budget, and at least one whatever the budget."""
     per = max(1, int(budget_rows) // (int(candidates) * int(Tw)))
     return [(w0, min(n_windows, w0 + per)) for w0 in range(0, n_windows, per)]
+
+
+# ---- stream groups (SAMAudio.stream_group, DESIGN.md section 3) ----
+# A tick advances several streams at once: the windows every stream makes ready are solved together, in the groups of
+# window_groups, and each planned call (encode, solve, decode) runs at an item count rounded up to a bucket, so that the
+# engine keeps one plan per bucket instead of planning anew whenever the number of windows in a tick changes.
+
+
+def stream_group_capacity(W: int, budget_rows: int) -> int:
+    """Items of the largest planned call of a stream group: the windows of one grouped solve.  A tick's encode and
+    decode calls of a group never have more items than the windows solved in it (one slice per window or per stream)."""
+    return max(1, int(budget_rows) // int(W))
+
+
+def stream_buckets(capacity: int) -> List[int]:
+    """The item counts a stream group plans calls for: the powers of two below capacity, then capacity."""
+    out, b = [], 1
+    while b < int(capacity):
+        out.append(b)
+        b *= 2
+    return out + [int(capacity)]
+
+
+def stream_bucket(n: int, capacity: int, resident: Sequence[int] = ()) -> List[int]:
+    """Slots of a planned call of n live items: the smallest power of two >= n, capped at capacity, or, when resident
+    bucket sizes are given and one of them is >= n, the smallest such (a flush reuses the plans of earlier ticks).
+    Slot i < n holds item i; every spare slot repeats a live item (item i % n) and its output is dropped.  An item's
+    result does not depend on the other items of its call, so the filler changes no bit."""
+    n, capacity = int(n), int(capacity)
+    if not 1 <= n <= capacity:
+        raise ValueError(f"a planned call of {n} items in a stream group of capacity {capacity}")
+    fits = [int(b) for b in resident if int(b) >= n]
+    size = min(fits) if fits else next(b for b in stream_buckets(capacity) if b >= n)
+    return [i % n for i in range(size)]
+
+
+def stream_flush_rows(budget_rows: int, W: int, resident: Sequence[int]) -> int:
+    """Row budget of the grouped solves of a flush tick: at most the largest resident bucket of windows, so that ending
+    many streams at once reuses the plans of the steady ticks instead of planning a larger bucket beside them."""
+    return min(int(budget_rows), max(resident) * int(W)) if resident else int(budget_rows)
+
+
+class TickWindows(NamedTuple):
+    key: object    # the stream
+    ka: int        # first window of the stream solved in this group
+    kb: int        # one past the last
+    last: bool     # kb is the stream's k_end of this tick
+
+
+def stream_tick_groups(due: Sequence[Tuple[object, int, int]], W: int, budget_rows: int) -> List[List[TickWindows]]:
+    """The grouped solves of a tick.  due = [(stream, k0, k_end)], the windows [k0, k_end) each stream solves in this
+    tick, in tick order.  Every window goes in order into groups of at most stream_group_capacity(W, budget_rows)
+    windows (the groups of window_groups over all of them); a stream's windows inside a group are one range."""
+    flat = [(key, k, k_end) for key, k0, k_end in due for k in range(int(k0), int(k_end))]
+    groups: List[List[TickWindows]] = []
+    for g0, g1 in window_groups(len(flat), 1, W, budget_rows):
+        grp: List[TickWindows] = []
+        for key, k, k_end in flat[g0:g1]:
+            if grp and grp[-1].key is key:
+                grp[-1] = grp[-1]._replace(kb=k + 1, last=k + 1 == k_end)
+            else:
+                grp.append(TickWindows(key, k, k + 1, k + 1 == k_end))
+        groups.append(grp)
+    return groups
