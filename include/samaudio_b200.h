@@ -239,6 +239,64 @@ int sab_test_attention_tc2(int items, int heads, int T, const void* q_bf16, cons
 int sab_test_attention_stream(int items, int heads, int T, const void* q_bf16, const void* k_bf16, const void* v_bf16,
                               const uint8_t* key_mask, void* o_bf16, float shift_log2, int poly, void* stream);
 
+/* The SIMT kernels of the DiT, codec and T5 paths, each through the launch helper the engine itself calls (same kernels,
+ * grids and variant choice).  Every argument rule is checked before any CUDA call; a refusal returns non-zero with the rule
+ * in sab_last_error().  All pointers are device addresses; fp32 unless stated.
+ *
+ * Fused RMSNorm + adaLN modulate (rmsnorm_mod_kernel<d/128>, d/128 in {2,4,8,12,16,20,22,24,32}), x [M, d]:
+ *   out[m, :] = bf16(x[m,:] * rsqrt(mean(x[m,:]^2) + eps) * w * (1 + scale[b,:]) + shift[b,:]),  b = m / rows_per_item,
+ *   shift / scale rows b at b * mod_ld (0: one row for all); reverse = 1 walks the rows last first (same values). */
+int sab_test_rmsnorm_mod(int M, int d, const float* x, const float* w, const float* shift, const float* scale,
+                         int64_t mod_ld, int rows_per_item, float eps, int reverse, void* out_bf16, void* stream);
+/* GroupNorm(1 group) + SiLU (gn_stats_kernel + gn_silu_kernel) of `items` slabs x [items, n_per_item] (C channels
+ * innermost): y = bf16(silu((x - mean) * rsqrt(var + eps) * gamma[c] + beta[c])), mean / biased var over the slab. */
+int sab_test_group_norm_silu(int items, int64_t n_per_item, int C, const float* x, const float* gamma, const float* beta,
+                             float eps, void* y_bf16, void* stream);
+/* Time features of R = B * cand sequences; each output may be NULL (its kernel is skipped):
+ *   tfreq [R, 256] bf16 = (cos, sin)(time[r] * exp(-ln(1e4) k / 128)), k < 128          (tfreq_kernel)
+ *   mem_in [R/cand * L, d] bf16 = mem_base + (cos, sin)(time[b*cand] * exp(-ln(1e4) k / (d/2)))   (mem_time_kernel)
+ *   mod [n_layers, R, 6, d] = tables[l] + t0[r] ([6, d] rows); fin [R, 2, d] = ftable + t[r]   (build_mod_kernel)
+ *   cs [2 n_layers, R, d] = norm_w[k] * (1 + mod[k/2, r, 3(k%2) + 1]); shift [2 n_layers, R, d] bf16 = bf16(mod[k/2, r,
+ *   3(k%2)])                                                                               (norm_tables_kernel) */
+int sab_test_time_features(int R, int cand, int d, int n_layers, int L, const float* time, void* tfreq_bf16,
+                           const float* mem_base, void* mem_in_bf16, const float* tables, const float* t0, const float* ftable,
+                           const float* t, float* mod, float* fin, const float* norm_w, float* cs, void* shift_bf16,
+                           void* stream);
+/* Conditioning finish of sab_prepare for M = B * cand * T sequence rows (flags: SAB_PREP_NO_VIDEO_TERM, SAB_PREP_NO_ANCHORS):
+ *   vconst = LayerNorm(vid_bias) * ln_w + ln_b (eps 1e-5)                                   (ln_vector_kernel)
+ *   anchor_table [n_anchor, d] = anchor_embed [n_anchor, anchor_dim] @ anchor_proj [d, anchor_dim]^T   (small_abt_kernel)
+ *   cond[m] = cond_clip[c] + tanh(gate_v) * (vproj ? LayerNorm(vproj[c]) * ln_w + ln_b : vconst)
+ *             + tanh(gate_a) * anchor_table[anchor_ids[b, anchor_align[c]]]                   (cond_finish_kernel)
+ *   with clip b = m / T / cand, clip row c = b * T + m % T; cond == cond_clip (in place) exactly when cand == 1. */
+int sab_test_cond_finish(int B, int cand, int T, int d, float* cond, const float* cond_clip, const float* vproj,
+                         const float* ln_w, const float* ln_b, const float* vid_bias, float* vconst, const float* gate_v,
+                         const float* anchor_embed, const float* anchor_proj, int n_anchor, int anchor_dim,
+                         float* anchor_table, const int64_t* anchor_ids, int n_ids, const int64_t* anchor_align,
+                         const float* gate_a, int flags, void* stream);
+/* RoPE table (rope_table_kernel): out [T, hd/2] (cos, sin) float pairs of pos * theta^(-2i/hd). */
+int sab_test_rope_table(int T, int hd, float theta, float* out, void* stream);
+/* The codec's 1-channel end layers; variant -1 = the engine's choice, 0 = the generic kernel, 1 = the register kernel.
+ *  which 0, encoder.block.0 (enc_conv0{,_reg}_kernel): in = wav [items, S], w [C, 7], bias [C], alpha [C]:
+ *    x_out [items, S, C] = bias[c] + sum_k w[c, k] wav[t + k - 3] (zero outside [0, S)); a_out bf16 = bf16(Snake_alpha(x_out))
+ *  which 1, decoder last conv (dec_last_kernel, dec_last_reg_kernel<C/32> for C = 64, 96, 128): in = a bf16 [items, S, C],
+ *    w [C, 7], bias [1]:  wav_out [items, S] = tanh(bias + sum_{k,c} w[c, k] a[t + k - 3, c]). */
+int sab_test_codec_end(int which, int variant, int items, int64_t S, int C, const void* in, const float* w,
+                       const float* bias, const float* alpha, float* x_out, void* a_out_bf16, float* wav_out, void* stream);
+/* Cross-attention through the engine's dispatcher (xattn_small_kernel for Tk <= 16, attention_kernel above), the `cand`
+ * query items of a clip sharing its text: O[i] = softmax(Q[i] K[i/cand]^T / sqrt(128) + mask[i/cand]) V[i/cand];
+ * q, o [items*Tq, heads*128], k, v [items/cand*Tk, heads*128] bf16, key_mask [items/cand, Tk] (1 = attend) or NULL. */
+int sab_test_attention_cross(int items, int heads, int Tq, int Tk, int cand, const void* q, const void* k, const void* v,
+                             const uint8_t* key_mask, void* o, void* stream);
+/* T5LayerNorm (t5_norm_kernel): y = x * rsqrt(mean(x^2) + eps) * w, x [rows, d]; out_bf16 and / or out_f32 (NULL: skipped). */
+int sab_test_t5_norm(int64_t rows, int d, const float* x, const float* w, float eps, void* out_bf16, float* out_f32,
+                     void* stream);
+/* T5 self-attention of sab_t5_forward (t5_bias_table_kernel + t5_attention_kernel), 1 <= L <= 512:
+ *   bias [H, 2L-1] = rel_bias_w[rel_bucket[delta], h] (rel_bias_w [buckets, H]);
+ *   out[b*L + i, h*64 + c] = bf16(sum_j softmax_j(q_i . k_j + bias[h, j - i + L - 1], mask[b, j]) v_j[c]),
+ *   q | k | v = qkv [B*L, 3*H*64] bf16 column blocks; no 1/sqrt(d) scaling. */
+int sab_test_t5_attention(int B, int L, int H, const void* qkv, const float* rel_bias_w, const int32_t* rel_bucket,
+                          float* bias, const uint8_t* mask, void* out_bf16, void* stream);
+
 /* Time tiling of long clips in the codec (decoder != 0: sab_decode, else sab_encode) for a clip of T latent frames under
  * the current workspace budget: halo_frames = latent frames of context an output frame needs on each side, derived from
  * the codec's layer list; tile_frames = length of the tiles the clip is cut into, 0 when it runs whole. */

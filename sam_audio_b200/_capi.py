@@ -84,6 +84,8 @@ EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
     "sab_workspace_bytes", "sab_set_plan_limits", "sab_plan_stats", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_blend_windows", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_test_rmsnorm_mod", "sab_test_group_norm_silu", "sab_test_time_features", "sab_test_cond_finish",
+    "sab_test_rope_table", "sab_test_codec_end", "sab_test_attention_cross", "sab_test_t5_norm", "sab_test_t5_attention",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
 ]
 
@@ -132,6 +134,16 @@ def lib() -> ctypes.CDLL:
         L.sab_blend_windows.argtypes = [vp, i32, i32, vp, vp, vp, i32, vp, i32, i32, vp]
         L.sab_test_aa_taps.argtypes = [i32, i32, i32, vp, vp, vp, vp]
         L.sab_test_solver_grid.argtypes = [i32, i32, i32, vp, vp]
+        f32 = ctypes.c_float
+        L.sab_test_rmsnorm_mod.argtypes = [i32, i32, vp, vp, vp, vp, i64, i32, f32, i32, vp, vp]
+        L.sab_test_group_norm_silu.argtypes = [i32, i64, i32, vp, vp, vp, f32, vp, vp]
+        L.sab_test_time_features.argtypes = [i32, i32, i32, i32, i32] + [vp] * 14
+        L.sab_test_cond_finish.argtypes = [i32, i32, i32, i32] + [vp] * 10 + [i32, i32, vp, vp, i32, vp, vp, i32, vp]
+        L.sab_test_rope_table.argtypes = [i32, i32, f32, vp, vp]
+        L.sab_test_codec_end.argtypes = [i32, i32, i32, i64, i32, vp, vp, vp, vp, vp, vp, vp, vp]
+        L.sab_test_attention_cross.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+        L.sab_test_t5_norm.argtypes = [i64, i32, vp, vp, f32, vp, vp, vp]
+        L.sab_test_t5_attention.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
         L.sab_t5_create.argtypes = [ctypes.POINTER(SabT5Config), i32, ctypes.POINTER(vp)]
         L.sab_t5_destroy.argtypes = [vp]
         L.sab_t5_load_weight.argtypes = [vp, ctypes.c_char_p, vp, ctypes.POINTER(i64), i32, i32, vp]

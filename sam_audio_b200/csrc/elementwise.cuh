@@ -166,6 +166,9 @@ __global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __r
 // ---------------------------------------------------------------------------------------------
 // GroupNorm(1 group) over the whole (T, C) slab of an item, then SiLU  (patcher.py:83-98, num_groups=1)
 // pass 1: per-item partial sums (double) ; pass 2: normalise + affine + SiLU -> bf16
+// The sums are taken about the item's first element K: var = E[(x-K)^2] - E[x-K]^2 keeps the cancellation of
+// E[x^2] - mean^2 away when the item's mean is large next to its spread (mean/std = 300 lost every significant digit
+// of the variance in the fp32 per-thread partials; about K the loss scales with ((mean-K)/std)^2 instead).
 // ---------------------------------------------------------------------------------------------
 constexpr int GN_CHUNKS = 32;
 __global__ void __launch_bounds__(256)
@@ -175,9 +178,11 @@ gn_stats_kernel(const float* __restrict__ x, long long n_per_item, double* __res
   const long long per = (n4 + GN_CHUNKS - 1) / GN_CHUNKS;
   const long long lo = chunk * per, hi = (lo + per < n4) ? lo + per : n4;
   const float4* xp = reinterpret_cast<const float4*>(x + item * n_per_item);
+  const float K = x[item * n_per_item];
   float s = 0.f, q = 0.f;
   for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-    const float4 v = xp[i];
+    float4 v = xp[i];
+    v.x -= K; v.y -= K; v.z -= K; v.w -= K;
     s += v.x + v.y + v.z + v.w;
     q += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
   }
@@ -206,9 +211,9 @@ gn_silu_kernel(const float* __restrict__ x, const double* __restrict__ partial, 
       a += partial[((long long)item * GN_CHUNKS + i) * 2];
       b += partial[((long long)item * GN_CHUNKS + i) * 2 + 1];
     }
-    const double mean = a / (double)n_per_item;
-    const double var = b / (double)n_per_item - mean * mean;
-    s_mean = (float)mean;
+    const double dm = a / (double)n_per_item;          // mean - K
+    const double var = b / (double)n_per_item - dm * dm;
+    s_mean = (float)((double)x[item * n_per_item] + dm);
     s_rstd = (float)(1.0 / sqrt((var > 0 ? var : 0) + (double)eps));
   }
   __syncthreads();

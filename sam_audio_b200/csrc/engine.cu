@@ -969,11 +969,15 @@ static void launch_rmsnorm(const float* x, const float* w, const float* shift, c
                            int rows_per_item, bf16* out, int M, float eps, int reverse, cudaStream_t st) {
   rmsnorm_mod_kernel<V><<<(M + 7) / 8, 256, 0, st>>>(x, w, shift, scale, mod_ld, rows_per_item, out, M, eps, reverse);
 }
-static void rmsnorm_mod(sab_engine* e, const float* x, const float* w, const float* shift, const float* scale,
-                        long long mod_ld, int rows_per_item, bf16* out, int M, cudaStream_t st, int reverse = 0) {
-  const int d = e->cfg.dim;
-  const float eps = e->cfg.norm_eps;
-  mark(e, st, "rmsnorm_mod", 0, (double)M * d * 6.0);
+static bool rmsnorm_dim_supported(int d) {
+  switch (d) {
+    case 256: case 512: case 1024: case 1536: case 2048: case 2560: case 2816: case 3072: case 4096: return true;
+    default: return false;
+  }
+}
+static void launch_rmsnorm_mod(int d, const float* x, const float* w, const float* shift, const float* scale,
+                               long long mod_ld, int rows_per_item, bf16* out, int M, float eps, int reverse,
+                               cudaStream_t st) {
   switch (d / 128) {
 #define SAB_RN(v) case v: launch_rmsnorm<v>(x, w, shift, scale, mod_ld, rows_per_item, out, M, eps, reverse, st); break;
     SAB_RN(2) SAB_RN(4) SAB_RN(8) SAB_RN(12) SAB_RN(16) SAB_RN(20) SAB_RN(22) SAB_RN(24) SAB_RN(32)
@@ -982,20 +986,41 @@ static void rmsnorm_mod(sab_engine* e, const float* x, const float* w, const flo
   }
   SAB_CUDA(cudaGetLastError());
 }
+static void rmsnorm_mod(sab_engine* e, const float* x, const float* w, const float* shift, const float* scale,
+                        long long mod_ld, int rows_per_item, bf16* out, int M, cudaStream_t st, int reverse = 0) {
+  const int d = e->cfg.dim;
+  mark(e, st, "rmsnorm_mod", 0, (double)M * d * 6.0);
+  launch_rmsnorm_mod(d, x, w, shift, scale, mod_ld, rows_per_item, out, M, e->cfg.norm_eps, reverse, st);
+}
 
-static void attention(sab_engine* e, const AttnParams& ap, int items, int heads, cudaStream_t st) {
+// GroupNorm(1) + SiLU of `items` slabs of n_per_item floats (C channels innermost) -> bf16; partial holds
+// items * GN_CHUNKS * 2 doubles
+static void launch_gn_stats(const float* x, int items, long long n_per_item, double* partial, cudaStream_t st) {
+  gn_stats_kernel<<<dim3(GN_CHUNKS, items), 256, 0, st>>>(x, n_per_item, partial);
+}
+static void launch_gn_apply(const float* x, int items, long long n_per_item, int C, const float* gamma, const float* beta,
+                            float eps, const double* partial, bf16* y, cudaStream_t st) {
+  gn_silu_kernel<<<dim3(64, items), 256, 0, st>>>(x, partial, gamma, beta, C, n_per_item, eps, y);
+}
+
+// the engine's attention dispatch: a handful of text tokens go to the HBM-bound warp-per-row kernel, the rest to the
+// flash-style one
+static bool attention_is_xattn_small(const AttnParams& ap) { return ap.Tk <= XATT_MAX_TK && ap.k != ap.q; }
+static void launch_attention(const AttnParams& ap, int items, int heads, cudaStream_t st) {
   ensure_dynamic_smem(reinterpret_cast<const void*>(attention_kernel), ATT_SMEM);
-  const double fl = 4.0 * items * heads * (double)ap.Tq * ap.Tk * 128;
-  if (ap.Tk <= XATT_MAX_TK && ap.k != ap.q) {   // a handful of text tokens: HBM-bound warp-per-row kernel
-    mark(e, st, "sdpa.cross", fl, (double)items * ap.Tq * heads * 128 * 4.0);
+  if (attention_is_xattn_small(ap)) {
     launch_xattn_small(ap, items, heads, st);
-    SAB_CUDA(cudaGetLastError());
-    return;
+  } else {
+    dim3 grid((ap.Tq + ATT_BQ - 1) / ATT_BQ, heads, items);
+    attention_kernel<<<grid, ATT_THREADS, ATT_SMEM, st>>>(ap);
   }
-  dim3 grid((ap.Tq + ATT_BQ - 1) / ATT_BQ, heads, items);
-  mark(e, st, ap.k == ap.q ? "sdpa.self" : "sdpa.cross", fl, 0);
-  attention_kernel<<<grid, ATT_THREADS, ATT_SMEM, st>>>(ap);
   SAB_CUDA(cudaGetLastError());
+}
+static void attention(sab_engine* e, const AttnParams& ap, int items, int heads, cudaStream_t st) {
+  const double fl = 4.0 * items * heads * (double)ap.Tq * ap.Tk * 128;
+  if (attention_is_xattn_small(ap)) mark(e, st, "sdpa.cross", fl, (double)items * ap.Tq * heads * 128 * 4.0);
+  else mark(e, st, ap.k == ap.q ? "sdpa.self" : "sdpa.cross", fl, 0);
+  launch_attention(ap, items, heads, st);
 }
 
 // algorithmic HBM bytes of one GEMM launch: operands once + every epilogue stream once (what a perfect kernel moves)
@@ -1103,21 +1128,56 @@ struct FinalSpec {
 };
 
 // the time-only part of an evaluation for the R rows of a TimeState (ts.time holds the R times)
+// launch shapes of the time-feature and conditioning kernels, shared by the engine and the unit-test seams
+static void launch_tfreq(const float* time, int R, bf16* tfreq, cudaStream_t st) {
+  tfreq_kernel<<<(R * 256 + 255) / 256, 256, 0, st>>>(time, R, tfreq);
+}
+static void launch_mem_time(const float* time, int Bc, int cand, int d, int L, const float* mem_base, bf16* mem_in,
+                            cudaStream_t st) {
+  mem_time_kernel<<<256, 256, 0, st>>>(time, Bc, cand, d, L, mem_base, mem_in);
+}
+static void launch_build_mod(const float* tables, const float* t0, float* mod, int NL, int R, int d, const float* ftable,
+                             const float* t, float* fin, cudaStream_t st) {
+  build_mod_kernel<<<512, 256, 0, st>>>(tables, t0, mod, NL, R, d, ftable, t, fin);
+}
+static void launch_norm_tables(const float* mod, const float* norm_w, int NL, int R, int d, float* cs, bf16* shift,
+                               cudaStream_t st) {
+  norm_tables_kernel<<<512, 256, 0, st>>>(mod, norm_w, NL, R, d, cs, shift);
+}
+static void launch_rope_table(float2* rope, int T, int hd, float theta, cudaStream_t st) {
+  rope_table_kernel<<<(T * (hd / 2) + 255) / 256, 256, 0, st>>>(rope, T, hd, theta);
+}
+static void launch_ln_vector(const float* x, const float* w, const float* b, int d, float* y, cudaStream_t st) {
+  ln_vector_kernel<<<1, 256, 0, st>>>(x, w, b, d, y);
+}
+static void launch_small_abt(const float* A, const float* B, float* C, int I, int J, int K, cudaStream_t st) {
+  small_abt_kernel<<<(I * J + 255) / 256, 256, 0, st>>>(A, B, C, I, J, K);
+}
+static void launch_cond_finish(float* cond, const float* cond_clip, int M, int d, int T, int cand, const float* vproj,
+                               const float* ln_w, const float* ln_b, const float* vconst, const float* gate_v,
+                               const float* anchor_table, const long long* anchor_ids, int n_ids,
+                               const long long* anchor_align, const float* gate_a, int video_term, int anchor_term,
+                               cudaStream_t st) {
+  cond_finish_kernel<<<(M + 7) / 8, 256, 0, st>>>(cond, cond_clip, M, d, T, cand, vproj, ln_w, ln_b, vconst, gate_v,
+                                                  anchor_table, anchor_ids, n_ids, anchor_align, gate_a, video_term,
+                                                  anchor_term);
+}
+
 static void run_time_state(sab_engine* e, DitPlan& p, TimeState& ts, cudaStream_t st) {
   const sab_config& c = e->cfg;
   const int d = c.dim, NL = c.n_layers, R = ts.R;
   mark(e, st, "time_features_kernel");
-  tfreq_kernel<<<(R * 256 + 255) / 256, 256, 0, st>>>(ts.time, R, ts.tfreq);
+  launch_tfreq(ts.time, R, ts.tfreq, st);
   gemm(e, ts.g_t13, st);
   gemm(e, ts.g_t2, st);
   mark(e, st, "silu_cast_kernel");
   silu_cast_kernel<<<64, 256, 0, st>>>(ts.t, ts.t_silu, (long long)R * d);
   gemm(e, ts.g_tb, st);
   mark(e, st, "build_mod_kernel");
-  build_mod_kernel<<<512, 256, 0, st>>>(e->tables, ts.t0, ts.mod, NL, R, d, e->final_table, ts.t, ts.fin);
+  launch_build_mod(e->tables, ts.t0, ts.mod, NL, R, d, e->final_table, ts.t, ts.fin, st);
   if (p.fused_norm) {
     mark(e, st, "norm_tables_kernel");
-    norm_tables_kernel<<<512, 256, 0, st>>>(ts.mod, e->norm_w_all, NL, R, d, ts.cs, ts.shift);
+    launch_norm_tables(ts.mod, e->norm_w_all, NL, R, d, ts.cs, ts.shift, st);
     for (int l = 0; l < NL; ++l) {
       gemm(e, ts.g_bias_qkv[l], st);
       gemm(e, ts.g_bias_w13[l], st);
@@ -1144,7 +1204,7 @@ static void dit_eval(sab_engine* e, const float* time_dev, const FinalSpec& fs, 
   };
 
   mark(e, st, "mem_time_kernel");
-  mem_time_kernel<<<256, 256, 0, st>>>(time_dev, Bc, cand, d, L, p.mem_base, p.mem_in);
+  launch_mem_time(time_dev, Bc, cand, d, L, p.mem_base, p.mem_in, st);
   gemm(e, p.g_y13, st);
   gemm(e, p.g_y2, st);
   gemm(e, p.g_in, st);
@@ -1152,10 +1212,9 @@ static void dit_eval(sab_engine* e, const float* time_dev, const FinalSpec& fs, 
   for (int b = 0; b < 2; ++b) {
     const float* src = b == 0 ? p.x0 : p.c1;
     mark(e, st, "gn_stats_kernel");
-    gn_stats_kernel<<<dim3(GN_CHUNKS, Bc), 256, 0, st>>>(src, (long long)T * d, p.gn_partial);
+    launch_gn_stats(src, Bc, (long long)T * d, p.gn_partial, st);
     mark(e, st, "gn_silu_kernel");
-    gn_silu_kernel<<<dim3(64, Bc), 256, 0, st>>>(src, p.gn_partial, e->xe_gn_w[b], e->xe_gn_b[b], d, (long long)T * d,
-                                               1e-5f, p.gn_a);
+    launch_gn_apply(src, Bc, (long long)T * d, d, e->xe_gn_w[b], e->xe_gn_b[b], 1e-5f, p.gn_partial, p.gn_a, st);
     GemmOp xe = p.g_xe[b];
     if (b == 1) bind_cs(xe, 0);
     gemm(e, xe, st);
@@ -1547,7 +1606,7 @@ int sab_create(const sab_config* cfg, int device, sab_engine** out) {
     register_weights(e);
     e->rope_len = cfg->max_positions;
     e->rope = reinterpret_cast<float2*>(e->wpool.alloc<float>((int64_t)e->rope_len * 64 * 2));
-    rope_table_kernel<<<(e->rope_len * 64 + 255) / 256, 256>>>(e->rope, e->rope_len, 128, cfg->rope_theta);
+    launch_rope_table(e->rope, e->rope_len, 128, cfg->rope_theta, 0);
     SAB_CUDA(cudaGetLastError());
     SAB_CUDA(cudaDeviceSynchronize());
   } catch (...) {
@@ -1620,11 +1679,10 @@ int sab_finalize_weights(sab_engine* e, int allow_missing, char* missing_out, in
   }
   const int d = e->cfg.dim;
   // constant video term for text-only prompts: LayerNorm(conv bias)   (SURVEY App. A.9)
-  ln_vector_kernel<<<1, 256, 0, st>>>(e->vid_b, e->vid_ln_w, e->vid_ln_b, d, e->vid_const);
+  launch_ln_vector(e->vid_b, e->vid_ln_w, e->vid_ln_b, d, e->vid_const, st);
   // anchor table: embed [n,128] @ proj^T [128,d]
   const int n = e->cfg.n_anchor_tokens;
-  small_abt_kernel<<<(n * d + 255) / 256, 256, 0, st>>>(e->anchor_embed, e->anchor_proj, e->anchor_table, n, d,
-                                                         e->cfg.anchor_dim);
+  launch_small_abt(e->anchor_embed, e->anchor_proj, e->anchor_table, n, d, e->cfg.anchor_dim, st);
   SAB_CUDA(cudaGetLastError());
   SAB_CUDA(cudaStreamSynchronize(st));
   for (size_t l = 0; l < e->layers.size(); ++l) {
@@ -1708,11 +1766,9 @@ int sab_prepare(sab_engine* e, int B, int candidates, int T, int L, const float*
     vproj = p.vproj;
   }
   mark(e, st, "cond_finish_kernel");
-  cond_finish_kernel<<<(int)((M + 7) / 8), 256, 0, st>>>(p.cond, p.condB, (int)M, d, T, candidates, vproj, e->vid_ln_w,
-                                                        e->vid_ln_b, e->vid_const, e->vid_gate, e->anchor_table,
-                                                        reinterpret_cast<const long long*>(p.anchor_ids), n_ids,
-                                                        reinterpret_cast<const long long*>(p.anchor_align), e->anchor_gate,
-                                                        (flags & SAB_PREP_NO_VIDEO_TERM) ? 0 : 1, no_anchor ? 0 : 1);
+  launch_cond_finish(p.cond, p.condB, (int)M, d, T, candidates, vproj, e->vid_ln_w, e->vid_ln_b, e->vid_const,
+                     e->vid_gate, e->anchor_table, p.anchor_ids, n_ids, p.anchor_align, e->anchor_gate,
+                     (flags & SAB_PREP_NO_VIDEO_TERM) ? 0 : 1, no_anchor ? 0 : 1, st);
   SAB_CUDA(cudaGetLastError());
   SAB_API_END
 }
@@ -1859,6 +1915,45 @@ int sab_solve(sab_engine* e, const float* noise, int n_steps, int method, float*
   SAB_API_END
 }
 
+// The codec's two 1-channel end layers (codec_kernels.cuh).  variant: -1 = the engine's choice (the register kernel
+// wherever it applies), 0 = the generic kernel, 1 = the register kernel; a variant that cannot take the shape throws.
+static bool enc_conv0_reg_ok(int C0) { return C0 >= 4 && C0 % 4 == 0 && 256 % (C0 / 4) == 0; }
+static void launch_enc_conv0(int variant, const float* wav, int items, long long S, int C0, const float* w,
+                             const float* bias, const float* alpha, float* x_out, bf16* a_out, cudaStream_t st) {
+  SAB_CHECK(C0 >= 4 && C0 % 4 == 0, "enc.conv0: C0=%d must be a positive multiple of 4", C0);
+  const bool reg = variant < 0 ? enc_conv0_reg_ok(C0) : variant == 1;
+  SAB_CHECK(!reg || enc_conv0_reg_ok(C0), "enc.conv0: the register kernel needs C0/4 to divide 256 (C0=%d)", C0);
+  if (reg) {
+    const long long per_block = (256 / (C0 / 4)) * ENC0_ITER;
+    enc_conv0_reg_kernel<<<dim3((unsigned)((S + per_block - 1) / per_block), items), 256, 0, st>>>(
+        wav, S, C0, w, bias, alpha, x_out, a_out);
+  } else {
+    const long long n = S * (C0 / 4);
+    enc_conv0_kernel<<<dim3((unsigned)((n + 255) / 256), items), 256, 0, st>>>(wav, S, C0, w, bias, alpha, x_out, a_out);
+  }
+  SAB_CUDA(cudaGetLastError());
+}
+static int dec_last_smem(int C) { return ((DEC_LAST_TB + 6) * (C + 2) + 2) * 2 + 7 * C * 4; }
+static bool dec_last_reg_ok(int C) { return C == 64 || C == 96 || C == 128; }
+static void launch_dec_last(int variant, const bf16* a, int items, long long S, int C, const float* w, const float* bias,
+                            float* wav, cudaStream_t st) {
+  SAB_CHECK(C >= 2 && C % 2 == 0, "dec.last: C=%d must be even", C);
+  const bool reg = variant < 0 ? dec_last_reg_ok(C) : variant == 1;
+  SAB_CHECK(!reg || dec_last_reg_ok(C), "dec.last: the register kernel takes C = 64, 96 or 128 (C=%d)", C);
+  SAB_CHECK(reg || dec_last_smem(C) <= 48 * 1024, "dec.last: C=%d needs %d B of shared memory (at most 49152)", C,
+            dec_last_smem(C));
+  if (reg) {
+    const dim3 rgrid((unsigned)((S + 32 * DEC_SEG - 1) / (32 * DEC_SEG)), items);
+    if (C == 96) dec_last_reg_kernel<3><<<rgrid, 256, 0, st>>>(a, S, w, bias, wav);
+    else if (C == 64) dec_last_reg_kernel<2><<<rgrid, 256, 0, st>>>(a, S, w, bias, wav);
+    else dec_last_reg_kernel<4><<<rgrid, 256, 0, st>>>(a, S, w, bias, wav);
+  } else {
+    dec_last_kernel<<<dim3((unsigned)((S + DEC_LAST_TB - 1) / DEC_LAST_TB), items), DEC_LAST_TB, dec_last_smem(C), st>>>(
+        a, S, C, w, bias, wav);
+  }
+  SAB_CUDA(cudaGetLastError());
+}
+
 static void run_codec(sab_engine* e, CodecPlan& cp, int items, const float* wav_in, const float* latent_in, int T,
                       float* out, cudaStream_t st) {
   const sab_config& c = e->cfg;
@@ -1866,16 +1961,9 @@ static void run_codec(sab_engine* e, CodecPlan& cp, int items, const float* wav_
     switch (s.kind) {
       case CodecStep::ENC0: {
         const int C0 = c.codec_encoder_dim;
-        const long long n = cp.S * (C0 / 4);
         mark(e, st, "codec.enc.conv0", 2.0 * items * (double)cp.S * C0 * 7, (double)items * cp.S * (4.0 + C0 * 6.0));
-        if (C0 % 4 == 0 && 256 % (C0 / 4) == 0) {
-          const long long per_block = (256 / (C0 / 4)) * ENC0_ITER;
-          enc_conv0_reg_kernel<<<dim3((unsigned)((cp.S + per_block - 1) / per_block), items), 256, 0, st>>>(
-              wav_in, cp.S, C0, e->enc0_w, e->enc0_b, e->enc_blocks[0].ru[0].a0, cp.x_first, cp.a_first);
-        } else {
-          enc_conv0_kernel<<<dim3((unsigned)((n + 255) / 256), items), 256, 0, st>>>(
-              wav_in, cp.S, C0, e->enc0_w, e->enc0_b, e->enc_blocks[0].ru[0].a0, cp.x_first, cp.a_first);
-        }
+        launch_enc_conv0(-1, wav_in, items, cp.S, C0, e->enc0_w, e->enc0_b, e->enc_blocks[0].ru[0].a0, cp.x_first,
+                         cp.a_first, st);
         break;
       }
       case CodecStep::LATENT_SPLIT: {
@@ -1886,15 +1974,8 @@ static void run_codec(sab_engine* e, CodecPlan& cp, int items, const float* wav_
       }
       case CodecStep::DEC_LAST: {
         const int C = c.codec_decoder_dim >> c.codec_n_rates;
-        const int smem = ((DEC_LAST_TB + 6) * (C + 2) + 2) * 2 + 7 * C * 4;
         mark(e, st, "codec.dec.last", 2.0 * items * (double)cp.S * C * 7, (double)items * cp.S * (4.0 + C * 2.0));
-        const dim3 rgrid((unsigned)((cp.S + 32 * DEC_SEG - 1) / (32 * DEC_SEG)), items);
-        if (C == 96) dec_last_reg_kernel<3><<<rgrid, 256, 0, st>>>(cp.a_last, cp.S, e->dec_last_w, e->dec_last_b, out);
-        else if (C == 64) dec_last_reg_kernel<2><<<rgrid, 256, 0, st>>>(cp.a_last, cp.S, e->dec_last_w, e->dec_last_b, out);
-        else if (C == 128) dec_last_reg_kernel<4><<<rgrid, 256, 0, st>>>(cp.a_last, cp.S, e->dec_last_w, e->dec_last_b, out);
-        else
-          dec_last_kernel<<<dim3((unsigned)((cp.S + DEC_LAST_TB - 1) / DEC_LAST_TB), items), DEC_LAST_TB, smem, st>>>(
-              cp.a_last, cp.S, C, e->dec_last_w, e->dec_last_b, out);
+        launch_dec_last(-1, cp.a_last, items, cp.S, C, e->dec_last_w, e->dec_last_b, out, st);
         break;
       }
       default: {
@@ -2319,6 +2400,154 @@ int sab_test_attention_stream(int items, int heads, int T, const void* q, const 
     throw;
   }
   g_attn_poly = saved;
+  SAB_API_END
+}
+
+// ---- SIMT kernel seams: each launches the engine's own helper (same kernels, grids and variant choice) ----
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+int sab_test_rmsnorm_mod(int M, int d, const float* x, const float* w, const float* shift, const float* scale,
+                         int64_t mod_ld, int rows_per_item, float eps, int reverse, void* out, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(x && w && shift && scale && out, "sab_test_rmsnorm_mod: null argument");
+  SAB_CHECK(rmsnorm_dim_supported(d), "sab_test_rmsnorm_mod: no instantiation for d=%d (d/128 in 2,4,8,12,16,20,22,24,32)", d);
+  SAB_CHECK(M >= 1 && rows_per_item >= 1, "sab_test_rmsnorm_mod: M=%d and rows_per_item=%d must be >= 1", M, rows_per_item);
+  SAB_CHECK(mod_ld >= 0 && mod_ld % 4 == 0, "sab_test_rmsnorm_mod: mod_ld=%lld must be a non-negative multiple of 4",
+            (long long)mod_ld);
+  SAB_CHECK(reverse == 0 || reverse == 1, "sab_test_rmsnorm_mod: reverse=%d must be 0 or 1", reverse);
+  SAB_CHECK(aligned16(x) && aligned16(w) && aligned16(shift) && aligned16(scale) && aligned16(out),
+            "sab_test_rmsnorm_mod: operands must be 16-byte aligned");
+  launch_rmsnorm_mod(d, x, w, shift, scale, (long long)mod_ld, rows_per_item, (bf16*)out, M, eps, reverse,
+                     (cudaStream_t)stream);
+  SAB_API_END
+}
+
+int sab_test_group_norm_silu(int items, int64_t n_per_item, int C, const float* x, const float* gamma,
+                             const float* beta, float eps, void* y, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(x && gamma && beta && y, "sab_test_group_norm_silu: null argument");
+  SAB_CHECK(items >= 1 && items <= 65535, "sab_test_group_norm_silu: items=%d outside 1..65535", items);
+  SAB_CHECK(C >= 4 && C % 4 == 0, "sab_test_group_norm_silu: C=%d must be a positive multiple of 4", C);
+  SAB_CHECK(n_per_item >= C && n_per_item % C == 0, "sab_test_group_norm_silu: n_per_item=%lld must be a multiple of C=%d",
+            (long long)n_per_item, C);
+  SAB_CHECK(aligned16(x) && aligned16(gamma) && aligned16(beta) && aligned16(y),
+            "sab_test_group_norm_silu: operands must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  double* partial = nullptr;
+  SAB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&partial), (size_t)items * GN_CHUNKS * 2 * sizeof(double), st));
+  launch_gn_stats(x, items, (long long)n_per_item, partial, st);
+  launch_gn_apply(x, items, (long long)n_per_item, C, gamma, beta, eps, partial, (bf16*)y, st);
+  const cudaError_t launched = cudaGetLastError();
+  SAB_CUDA(cudaFreeAsync(partial, st));
+  SAB_CUDA(launched);
+  SAB_API_END
+}
+
+int sab_test_time_features(int R, int cand, int d, int n_layers, int L, const float* time, void* tfreq,
+                           const float* mem_base, void* mem_in, const float* tables, const float* t0, const float* ftable,
+                           const float* t, float* mod, float* fin, const float* norm_w, float* cs, void* shift,
+                           void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(R >= 1 && cand >= 1 && R % cand == 0, "sab_test_time_features: R=%d must be a positive multiple of cand=%d",
+            R, cand);
+  SAB_CHECK(d >= 4 && d % 4 == 0 && n_layers >= 1 && L >= 1,
+            "sab_test_time_features: d=%d must be a positive multiple of 4, n_layers=%d and L=%d >= 1", d, n_layers, L);
+  SAB_CHECK(time || (!tfreq && !mem_in), "sab_test_time_features: tfreq / mem_in need time");
+  SAB_CHECK(!mem_in || mem_base, "sab_test_time_features: mem_in needs mem_base");
+  SAB_CHECK(!mod || (tables && t0 && ftable && t && fin), "sab_test_time_features: mod needs tables, t0, ftable, t and fin");
+  SAB_CHECK(!cs || (mod && norm_w && shift), "sab_test_time_features: cs needs mod, norm_w and shift");
+  SAB_CHECK(aligned16(tables) && aligned16(t0) && aligned16(ftable) && aligned16(t) && aligned16(mod) && aligned16(fin) &&
+            aligned16(norm_w) && aligned16(cs) && aligned16(shift),
+            "sab_test_time_features: table operands must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tfreq) launch_tfreq(time, R, (bf16*)tfreq, st);
+  if (mem_in) launch_mem_time(time, R, cand, d, L, mem_base, (bf16*)mem_in, st);
+  if (mod) launch_build_mod(tables, t0, mod, n_layers, R, d, ftable, t, fin, st);
+  if (cs) launch_norm_tables(mod, norm_w, n_layers, R, d, cs, (bf16*)shift, st);
+  SAB_CUDA(cudaGetLastError());
+  SAB_API_END
+}
+
+int sab_test_cond_finish(int B, int cand, int T, int d, float* cond, const float* cond_clip, const float* vproj,
+                         const float* ln_w, const float* ln_b, const float* vid_bias, float* vconst, const float* gate_v,
+                         const float* anchor_embed, const float* anchor_proj, int n_anchor, int anchor_dim,
+                         float* anchor_table, const int64_t* anchor_ids, int n_ids, const int64_t* anchor_align,
+                         const float* gate_a, int flags, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(cond && cond_clip && ln_w && ln_b && vid_bias && vconst && gate_v && anchor_embed && anchor_proj &&
+            anchor_table && gate_a, "sab_test_cond_finish: null argument");
+  SAB_CHECK(B >= 1 && cand >= 1 && T >= 1 && d >= 1, "sab_test_cond_finish: bad shape (B=%d, cand=%d, T=%d, d=%d)", B,
+            cand, T, d);
+  SAB_CHECK((int64_t)B * cand * T < (1LL << 31) - 8, "sab_test_cond_finish: B * cand * T rows exceed the int range");
+  SAB_CHECK((cand == 1) == (cond == cond_clip), "sab_test_cond_finish: cond aliases cond_clip exactly when cand == 1");
+  SAB_CHECK(n_anchor >= 1 && anchor_dim >= 1, "sab_test_cond_finish: n_anchor=%d and anchor_dim=%d must be >= 1",
+            n_anchor, anchor_dim);
+  const bool anchors = (flags & SAB_PREP_NO_ANCHORS) == 0;
+  SAB_CHECK(!anchors || (anchor_ids && anchor_align && n_ids >= 1), "sab_test_cond_finish: anchor tensors missing");
+  SAB_CHECK((flags & ~(SAB_PREP_NO_VIDEO_TERM | SAB_PREP_NO_ANCHORS)) == 0, "sab_test_cond_finish: unknown flags %d",
+            flags);
+  cudaStream_t st = (cudaStream_t)stream;
+  launch_ln_vector(vid_bias, ln_w, ln_b, d, vconst, st);
+  launch_small_abt(anchor_embed, anchor_proj, anchor_table, n_anchor, d, anchor_dim, st);
+  launch_cond_finish(cond, cond_clip, B * cand * T, d, T, cand, vproj, ln_w, ln_b, vconst, gate_v, anchor_table,
+                     reinterpret_cast<const long long*>(anchor_ids), n_ids,
+                     reinterpret_cast<const long long*>(anchor_align), gate_a,
+                     (flags & SAB_PREP_NO_VIDEO_TERM) ? 0 : 1, anchors ? 1 : 0, st);
+  SAB_CUDA(cudaGetLastError());
+  SAB_API_END
+}
+
+int sab_test_rope_table(int T, int hd, float theta, float* out, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(out, "sab_test_rope_table: null argument");
+  SAB_CHECK(T >= 1 && hd >= 2 && hd % 2 == 0 && (int64_t)T * (hd / 2) < (1LL << 31) - 256,
+            "sab_test_rope_table: bad shape (T=%d, hd=%d)", T, hd);
+  SAB_CHECK(theta > 1.f, "sab_test_rope_table: theta=%g must be > 1", theta);
+  launch_rope_table(reinterpret_cast<float2*>(out), T, hd, theta, (cudaStream_t)stream);
+  SAB_CUDA(cudaGetLastError());
+  SAB_API_END
+}
+
+int sab_test_codec_end(int which, int variant, int items, int64_t S, int C, const void* in, const float* w,
+                       const float* bias, const float* alpha, float* x_out, void* a_out, float* wav_out, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(which == 0 || which == 1, "sab_test_codec_end: which=%d must be 0 (enc.conv0) or 1 (dec.last)", which);
+  SAB_CHECK(variant >= -1 && variant <= 1, "sab_test_codec_end: variant=%d must be -1, 0 or 1", variant);
+  SAB_CHECK(items >= 1 && items <= 65535 && S >= 1, "sab_test_codec_end: bad shape (items=%d, S=%lld)", items,
+            (long long)S);
+  SAB_CHECK(in && w && bias, "sab_test_codec_end: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (which == 0) {
+    SAB_CHECK(alpha && x_out && a_out, "sab_test_codec_end: enc.conv0 needs alpha, x_out and a_out");
+    SAB_CHECK(aligned16(x_out) && ((uintptr_t)a_out & 7) == 0, "sab_test_codec_end: x_out / a_out misaligned");
+    SAB_CHECK(S * (C / 4) / 256 < (1LL << 31), "sab_test_codec_end: S=%lld too long for one launch", (long long)S);
+    launch_enc_conv0(variant, (const float*)in, items, S, C, w, bias, alpha, x_out, (bf16*)a_out, st);
+  } else {
+    SAB_CHECK(wav_out, "sab_test_codec_end: dec.last needs wav_out");
+    SAB_CHECK(((uintptr_t)in & 7) == 0, "sab_test_codec_end: the bf16 input must be 8-byte aligned");
+    launch_dec_last(variant, (const bf16*)in, items, S, C, w, bias, wav_out, st);
+  }
+  SAB_API_END
+}
+
+int sab_test_attention_cross(int items, int heads, int Tq, int Tk, int cand, const void* q, const void* k, const void* v,
+                             const uint8_t* key_mask, void* o, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(q && k && v && o, "sab_test_attention_cross: null argument");
+  SAB_CHECK(k != q, "sab_test_attention_cross: k == q selects self-attention");
+  SAB_CHECK(items >= 1 && items <= 65535 && heads >= 1 && heads <= 65535 && Tq >= 1 && Tk >= 1,
+            "sab_test_attention_cross: bad shape (items=%d, heads=%d, Tq=%d, Tk=%d)", items, heads, Tq, Tk);
+  SAB_CHECK(cand >= 1 && items % cand == 0, "sab_test_attention_cross: items=%d must be a multiple of cand=%d", items,
+            cand);
+  SAB_CHECK(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o), "sab_test_attention_cross: operands must be "
+            "16-byte aligned");
+  AttnParams a{};
+  const long long ld = (long long)heads * 128;
+  a.q = (const bf16*)q; a.q_ld = ld; a.k = (const bf16*)k; a.k_ld = ld; a.v = (const bf16*)v; a.v_ld = ld;
+  a.o = (bf16*)o; a.o_ld = ld; a.key_mask = key_mask; a.Tq = Tq; a.Tk = Tk;
+  a.scale_log2 = (1.0f / sqrtf(128.f)) * 1.4426950408889634f;
+  a.kv_div = cand; a.mask_div = cand;
+  launch_attention(a, items, heads, (cudaStream_t)stream);
   SAB_API_END
 }
 

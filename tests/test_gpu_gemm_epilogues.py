@@ -25,7 +25,7 @@ import sys
 import pytest
 import torch
 
-from _util import rel_l2
+from _util import rel_l2, snake_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -100,12 +100,6 @@ def assert_close(o, r, what, bf16=False, extra=0.0, rms=None):
 
 def snake(v, a):
     return v + torch.sin(a * v) ** 2 / (a + 1e-9)
-
-
-def snake_bound(v, a):
-    """|__sinf / rcp.approx Snake - exact| for input v, alpha a (module docstring)."""
-    d_sin = 2.0 ** -21.41 + 2.0 ** -22 * (a * v).abs()
-    return (2 * d_sin + 2.0 ** -21) / a
 
 
 def bf16_mismatch_bound(m, delta):
