@@ -323,6 +323,35 @@ int sab_preprocess_frames(const uint8_t* frames, int n_frames, int H, int W, int
 #define SAB_WIN_LAST 2
 int sab_blend_windows(const float* win_latent, int n_win, int Tw, const int32_t* win_seq, const int32_t* win_start,
                       const uint8_t* win_flags, int ramp, float* latent, int Bc, int T, void* stream);
+/* Resampling.  replaces: torchaudio.functional.resample (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99), which
+ * the reference's processor applies to files; streams and SAMAudio.resample() use it to bring audio at any rate to the
+ * codec's rate and back (DESIGN.md section 3).  With g = gcd(orig, new), o = orig / g, n = new / g, output
+ * q = m * n + j (j < n) is y[q] = sum_{k < K} w[j][k] * x[m * o + lo[j] + k], a K-term fp32 FMA chain in ascending k;
+ * input samples outside [0, length) are zero and the output length is ceil(n * length / o).  orig == new is the
+ * identity (K = 1, w = 1).  The table of each rate pair is built on first use and kept, counted in sab_workspace_bytes,
+ * until sab_destroy.  One call runs every segment in one launch; an output's bits depend only on the signal and the
+ * table, never on how the outputs are split into segments.
+ *  Each segment: rates in [8000, 192000], 1 <= channels <= 8; input [channels, in_count] at channel stride
+ *  in_channel_stride holds signal samples [in_first, in_first + in_count), and the mono signal is their channel mean
+ *  (summed in ascending channel order, then divided by channels); length < 0 = not known yet, in which case only
+ *  negative indices read as zero; outputs [out_first, out_first + out_count) go to out (contiguous fp32).  Every input
+ *  index an output reads inside [0, length) must lie in the buffer.  Every rule is checked on the host before any CUDA
+ *  call; the descriptors go to the device asynchronously on `stream` (calls of one engine must be ordered on one
+ *  stream).  Not for graph capture. */
+typedef struct sab_resample_seg {
+  int32_t struct_bytes;     /* = sizeof(sab_resample_seg), checked first */
+  int32_t orig_rate, new_rate, channels;
+  const float* in;
+  int64_t in_channel_stride, in_first, in_count;
+  int64_t length;
+  float* out;
+  int64_t out_first, out_count;
+} sab_resample_seg;
+int sab_resample(sab_engine* e, const sab_resample_seg* segs, int n_segs, void* stream);
+/* Host-only: the table sab_resample uses for a rate pair: *K taps, lo [n] (n = new / gcd) and, when w is not NULL,
+ * w [n, K] fp32 (cap = floats w holds).  lo and w may be NULL to query K alone. */
+int sab_resample_taps(int orig_rate, int new_rate, int64_t cap, int* K, int* lo, float* w);
+
 /* host-only test seam: evaluation times of sab_solve's grid (method = SAB_ODE_*), in evaluation order */
 int sab_test_solver_grid(int method, int n_steps, int cap, int* n_evals, float* times);
 /* host-only test seam: tap window start / count / normalised weights ([out_size, cap], zero padded) of one axis */

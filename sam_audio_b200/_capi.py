@@ -80,10 +80,27 @@ class SabTestGemmDesc(ctypes.Structure):
             setattr(self, k, v)
 
 
+class SabResampleSeg(ctypes.Structure):
+    """Mirror of sab_resample_seg (include/samaudio_b200.h); pointers are device addresses as ints."""
+    _i32, _i64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
+    _fields_ = [("struct_bytes", _i32), ("orig_rate", _i32), ("new_rate", _i32), ("channels", _i32),
+                ("in_", _vp), ("in_channel_stride", _i64), ("in_first", _i64), ("in_count", _i64),
+                ("length", _i64),
+                ("out", _vp), ("out_first", _i64), ("out_count", _i64)]
+
+    def __init__(self, **kw):
+        super().__init__()
+        self.struct_bytes = ctypes.sizeof(SabResampleSeg)
+        self.channels, self.length = 1, -1
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
     "sab_workspace_bytes", "sab_set_plan_limits", "sab_plan_stats", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_blend_windows", "sab_test_aa_taps", "sab_test_solver_grid",
+    "sab_resample", "sab_resample_taps",
     "sab_test_rmsnorm_mod", "sab_test_group_norm_silu", "sab_test_time_features", "sab_test_cond_finish",
     "sab_test_rope_table", "sab_test_codec_end", "sab_test_attention_cross", "sab_test_t5_norm", "sab_test_t5_attention",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
@@ -134,6 +151,8 @@ def lib() -> ctypes.CDLL:
         L.sab_blend_windows.argtypes = [vp, i32, i32, vp, vp, vp, i32, vp, i32, i32, vp]
         L.sab_test_aa_taps.argtypes = [i32, i32, i32, vp, vp, vp, vp]
         L.sab_test_solver_grid.argtypes = [i32, i32, i32, vp, vp]
+        L.sab_resample.argtypes = [vp, ctypes.POINTER(SabResampleSeg), i32, vp]
+        L.sab_resample_taps.argtypes = [i32, i32, i64, ctypes.POINTER(i32), vp, vp]
         f32 = ctypes.c_float
         L.sab_test_rmsnorm_mod.argtypes = [i32, i32, vp, vp, vp, vp, i64, i32, f32, i32, vp, vp]
         L.sab_test_group_norm_silu.argtypes = [i32, i64, i32, vp, vp, vp, f32, vp, vp]
@@ -223,6 +242,28 @@ def blend_windows(win_latent: torch.Tensor, seq: torch.Tensor, start: torch.Tens
     return out
 
 
+def resample_taps(orig_rate: int, new_rate: int):
+    """The table sab_resample uses for a rate pair (host only): (K, lo [n] int32, w [n, K] fp32) as numpy arrays."""
+    import math
+
+    import numpy as np
+    n = int(new_rate) // math.gcd(int(orig_rate), int(new_rate))
+    K = ctypes.c_int()
+    check(lib().sab_resample_taps(int(orig_rate), int(new_rate), 0, ctypes.byref(K), None, None))
+    lo = np.zeros(n, np.int32)
+    w = np.zeros((n, K.value), np.float32)
+    check(lib().sab_resample_taps(int(orig_rate), int(new_rate), w.size, ctypes.byref(K), lo.ctypes.data, w.ctypes.data))
+    return K.value, lo, w
+
+
+def resample_segments(segs) -> ctypes.Array:
+    """A list of SabResampleSeg (or of dicts of its fields) as the C array sab_resample takes."""
+    arr = (SabResampleSeg * max(1, len(segs)))()
+    for i, s in enumerate(segs):
+        arr[i] = s if isinstance(s, SabResampleSeg) else SabResampleSeg(**s)
+    return arr
+
+
 class Engine:
     """Owns one sab_engine handle."""
 
@@ -299,6 +340,11 @@ class Engine:
 
     def workspace_bytes(self) -> int:
         return int(lib().sab_workspace_bytes(self._h))
+
+    def resample(self, segs) -> None:
+        """One sab_resample launch over `segs` (SabResampleSeg or dicts of its fields) on the current stream."""
+        if segs:
+            check(lib().sab_resample(self._h, resample_segments(segs), len(segs), stream_ptr()))
 
     DEFAULT_PLAN_LIMITS = (1, 3)    # include/samaudio_b200.h sab_set_plan_limits
 

@@ -21,6 +21,7 @@
 #include "vision_kernels.cuh"
 #include "xattn_fold.cuh"
 #include "blend_windows.cuh"
+#include "resample.cuh"
 
 using namespace sab;
 typedef __nv_bfloat16 bf16;
@@ -375,6 +376,7 @@ struct DecBlockW { float* a_up; ConvLayer up; ResUnitW ru[3]; int cin, cout, str
 
 struct DitPlan;
 struct CodecPlan;
+struct ResampleTableDev { DevicePool pool; int o = 1, n = 1, K = 1; float* w = nullptr; int* lo = nullptr; };
 struct ProfRec { const char* tag; double flops; double bytes; };
 
 struct sab_engine {
@@ -423,6 +425,12 @@ struct sab_engine {
   int64_t plan_clock = 0;
   size_t max_dit_plans = 1, max_codec_plans = 3;   // sab_set_plan_limits
   int64_t dit_plan_builds = 0, graph_captures = 0, codec_plan_builds = 0;   // sab_plan_stats
+
+  // sab_resample: one table per rate pair, kept until sab_destroy, and the device copy of a call's segment list
+  std::map<std::pair<int, int>, std::unique_ptr<ResampleTableDev>> rs_tables;
+  DevicePool rs_desc_pool;
+  ResampleSeg* rs_desc = nullptr;
+  int64_t rs_desc_cap = 0;
 
   ~sab_engine();
 };
@@ -2156,7 +2164,8 @@ int64_t sab_workspace_bytes(sab_engine* e) {
   for (auto& p : e->dit_plans) b += p->pool.bytes;
   for (auto& kv : e->enc_plans) b += kv.second->pool.bytes;
   for (auto& kv : e->dec_plans) b += kv.second->pool.bytes;
-  return b;
+  for (auto& kv : e->rs_tables) b += kv.second->pool.bytes;
+  return b + e->rs_desc_pool.bytes;
 }
 
 int sab_set_plan_limits(sab_engine* e, int dit_plans, int codec_plans_per_direction) {
@@ -2656,6 +2665,166 @@ int sab_blend_windows(const float* win_latent, int n_win, int Tw, const int32_t*
   BlendParams bp{win_latent, win_seq, win_start, win_flags, n_win, Tw, ramp, latent, T};
   const int per_cta = BW_WARPS * BW_FRAMES;
   blend_windows_kernel<<<dim3((T + per_cta - 1) / per_cta, Bc), BW_WARPS * 32, 0, (cudaStream_t)stream>>>(bp);
+  SAB_CUDA(cudaGetLastError());
+  SAB_API_END
+}
+
+// ---- resampling (resample.cuh) ----
+static int64_t floor_div(int64_t a, int64_t b) { return a / b - ((a % b != 0) && ((a < 0) != (b < 0))); }
+static int64_t ceil_div(int64_t a, int64_t b) { return -floor_div(-a, b); }
+
+// The polyphase table of torchaudio's sinc_interp_hann design (lowpass_filter_width 6, rolloff 0.99), evaluated in
+// float64 and rounded once to fp32.  With base = 0.99 min(o, n) and R = 6 o / base = 600 o / (99 min(o, n)), an exact
+// rational, K = 2 ceil(R) + 1 and lo[j] is the first integer i with i / o - j / n >= -R / o; both come from integer
+// arithmetic, so no rounding decides which taps a phase has.  w[j][k] = sinc(pi t) cos^2(pi t / 12) base / o with
+// t = clamp((lo[j] + k) / o - j / n, +-6 / base) base.
+struct ResampleTable { int o = 1, n = 1, K = 1; std::vector<int> lo; std::vector<float> w; };
+static bool resample_rate_ok(int r) { return r >= 8000 && r <= 192000; }
+static ResampleTable resample_table(int orig, int nw) {
+  ResampleTable t;
+  if (orig == nw) {                                  // the identity, as in torchaudio: no filter
+    t.lo = {0};
+    t.w = {1.f};
+    return t;
+  }
+  int64_t a = orig, b = nw;
+  while (b) { const int64_t r = a % b; a = b; b = r; }
+  const int64_t o = orig / a, n = nw / a, mn = o < n ? o : n;
+  const int64_t den = 99 * mn;                       // R = 600 o / den
+  t.o = (int)o; t.n = (int)n;
+  t.K = (int)(2 * ceil_div(600 * o, den) + 1);
+  t.lo.resize(n);
+  t.w.resize((size_t)n * t.K);
+  const double base = 0.99 * (double)mn, pi = 3.14159265358979323846;
+  for (int64_t j = 0; j < n; ++j) {
+    // i n den >= j o den - 600 o n
+    const int64_t lo = ceil_div(j * o * den - 600 * o * n, n * den);
+    t.lo[j] = (int)lo;
+    for (int k = 0; k < t.K; ++k) {
+      double x = (double)((lo + k) * n - j * o) / ((double)o * (double)n) * base;
+      x = x < -6.0 ? -6.0 : (x > 6.0 ? 6.0 : x);
+      const double c = cos(x * pi / 12.0);
+      const double s = x == 0.0 ? 1.0 : sin(pi * x) / (pi * x);
+      t.w[(size_t)j * t.K + k] = (float)(s * (c * c * base / (double)o));
+    }
+  }
+  return t;
+}
+
+static const ResampleTableDev& resample_table_dev(sab_engine* e, int orig, int nw) {
+  auto& slot = e->rs_tables[{orig, nw}];
+  if (!slot) {
+    const ResampleTable h = resample_table(orig, nw);
+    auto d = std::make_unique<ResampleTableDev>();
+    d->o = h.o; d->n = h.n; d->K = h.K;
+    d->w = d->pool.alloc<float>((int64_t)h.w.size());
+    d->lo = d->pool.alloc<int>((int64_t)h.lo.size());
+    std::vector<float> wt(h.w.size());                 // k-major on the device: a warp's phases read adjacent floats
+    for (int j = 0; j < h.n; ++j)
+      for (int k = 0; k < h.K; ++k) wt[(size_t)k * h.n + j] = h.w[(size_t)j * h.K + k];
+    SAB_CUDA(cudaMemcpy(d->w, wt.data(), wt.size() * sizeof(float), cudaMemcpyHostToDevice));
+    SAB_CUDA(cudaMemcpy(d->lo, h.lo.data(), h.lo.size() * sizeof(int), cudaMemcpyHostToDevice));
+    slot = std::move(d);
+  }
+  return *slot;
+}
+
+int sab_resample_taps(int orig_rate, int new_rate, int64_t cap, int* K, int* lo, float* w) {
+  SAB_API_BEGIN
+  SAB_CHECK(K, "null argument");
+  SAB_CHECK(resample_rate_ok(orig_rate) && resample_rate_ok(new_rate), "rates %d -> %d: both must lie in [8000, 192000]",
+            orig_rate, new_rate);
+  const ResampleTable t = resample_table(orig_rate, new_rate);
+  *K = t.K;
+  if (lo) memcpy(lo, t.lo.data(), t.lo.size() * sizeof(int));
+  if (w) {
+    SAB_CHECK(cap >= (int64_t)t.w.size(), "tap capacity %lld < %zu", (long long)cap, t.w.size());
+    memcpy(w, t.w.data(), t.w.size() * sizeof(float));
+  }
+  SAB_API_END
+}
+
+int sab_resample(sab_engine* e, const sab_resample_seg* segs, int n_segs, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(n_segs >= 0 && (segs || n_segs == 0), "bad segment list (n_segs=%d)", n_segs);
+  // every rule on the host first: tables are built from integer rules alone, so the tap spans are known here
+  std::vector<ResampleTable> tabs;
+  std::map<std::pair<int, int>, size_t> tab_of;
+  for (int i = 0; i < n_segs; ++i) {
+    const sab_resample_seg& g = segs[i];
+    SAB_CHECK(g.struct_bytes == (int32_t)sizeof(sab_resample_seg),
+              "sab_resample_seg.struct_bytes=%d but the library's descriptor has %d bytes (header and binding differ)",
+              g.struct_bytes, (int)sizeof(sab_resample_seg));
+    SAB_CHECK(resample_rate_ok(g.orig_rate) && resample_rate_ok(g.new_rate),
+              "segment %d: rates %d -> %d: both must lie in [8000, 192000]", i, g.orig_rate, g.new_rate);
+    SAB_CHECK(g.channels >= 1 && g.channels <= 8, "segment %d: channels=%d outside 1..8", i, g.channels);
+    SAB_CHECK(g.in_count >= 0 && g.out_count >= 0 && g.out_first >= 0 && g.length >= -1,
+              "segment %d: negative count (in_count=%lld, out_first=%lld, out_count=%lld, length=%lld)", i,
+              (long long)g.in_count, (long long)g.out_first, (long long)g.out_count, (long long)g.length);
+    SAB_CHECK(g.channels == 1 || g.in_channel_stride >= g.in_count, "segment %d: channel stride %lld < in_count %lld", i,
+              (long long)g.in_channel_stride, (long long)g.in_count);
+    if (g.out_count == 0) continue;
+    SAB_CHECK(g.out != nullptr, "segment %d: null output", i);
+    const std::pair<int, int> key{g.orig_rate, g.new_rate};
+    if (!tab_of.count(key)) {
+      tab_of[key] = tabs.size();
+      tabs.push_back(resample_table(g.orig_rate, g.new_rate));
+    }
+    const ResampleTable& t = tabs[tab_of[key]];
+    if (g.length >= 0) {
+      const int64_t n_out = ceil_div((int64_t)t.n * g.length, t.o);
+      SAB_CHECK(g.out_first + g.out_count <= n_out, "segment %d: outputs [%lld, %lld) past the %lld of a %lld-sample signal",
+                i, (long long)g.out_first, (long long)(g.out_first + g.out_count), (long long)n_out, (long long)g.length);
+    }
+    const int64_t q0 = g.out_first, q1 = g.out_first + g.out_count - 1;
+    int64_t a = (q0 / t.n) * t.o + t.lo[q0 % t.n];
+    int64_t b = (q1 / t.n) * t.o + t.lo[q1 % t.n] + t.K;
+    a = a < 0 ? 0 : a;
+    if (g.length >= 0) b = b < g.length ? b : g.length;
+    if (a < b) {
+      SAB_CHECK(g.in != nullptr, "segment %d: null input", i);
+      SAB_CHECK(a >= g.in_first && b <= g.in_first + g.in_count,
+                "segment %d: outputs [%lld, %lld) read input samples [%lld, %lld), the buffer holds [%lld, %lld)", i,
+                (long long)q0, (long long)(q1 + 1), (long long)a, (long long)b, (long long)g.in_first,
+                (long long)(g.in_first + g.in_count));
+    }
+    SAB_CHECK(g.out_count <= (int64_t)RS_BLOCK * (INT32_MAX / 2), "segment %d: %lld outputs is too many for one call", i,
+              (long long)g.out_count);
+  }
+  SAB_CHECK(e != nullptr, "null engine");
+  DeviceGuard _dg(e->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<ResampleSeg> dev;
+  int64_t ctas = 0, tab_floats = 0, span = 0;
+  double bytes = 0;
+  for (int i = 0; i < n_segs; ++i) {
+    const sab_resample_seg& g = segs[i];
+    if (g.out_count == 0) continue;
+    const ResampleTableDev& t = resample_table_dev(e, g.orig_rate, g.new_rate);
+    ResampleSeg s{g.in, g.in_channel_stride, g.in_first, g.in_count, g.length, g.out, g.out_first, g.out_count,
+                  t.w, t.lo, t.o, t.n, t.K, g.channels, (int)ctas, (int64_t)t.n * t.K <= RS_SMEM_TABLE};
+    dev.push_back(s);
+    ctas += (g.out_count + RS_BLOCK - 1) / RS_BLOCK;
+    if (s.smem_table) tab_floats = std::max<int64_t>(tab_floats, (int64_t)t.n * t.K);
+    // a CTA's outputs q0 .. q0 + RS_BLOCK - 1 read m o + lo[j] within [q o / n - R, q o / n - R + 1) from the first
+    // to K past the last
+    span = std::max<int64_t>(span, ceil_div((int64_t)(RS_BLOCK - 1) * t.o, t.n) + t.K + 2);
+    bytes += 4.0 * (double)g.out_count * (1.0 + (double)g.channels * t.o / t.n);
+  }
+  SAB_CHECK(ctas <= INT32_MAX, "%lld CTAs is too many for one call", (long long)ctas);
+  if (dev.empty()) return 0;
+  const int64_t smem = (tab_floats + span) * (int64_t)sizeof(float);
+  SAB_CHECK(smem <= RS_MAX_SMEM, "resampling needs %lld B of shared memory (at most %d)", (long long)smem, RS_MAX_SMEM);
+  if ((int64_t)dev.size() > e->rs_desc_cap) {
+    SAB_CUDA(cudaStreamSynchronize(st));           // the old list may still be read by an earlier launch
+    e->rs_desc_pool.release();
+    e->rs_desc_cap = std::max<int64_t>(64, (int64_t)dev.size());
+    e->rs_desc = e->rs_desc_pool.alloc<ResampleSeg>(e->rs_desc_cap);
+  }
+  SAB_CUDA(cudaMemcpyAsync(e->rs_desc, dev.data(), dev.size() * sizeof(ResampleSeg), cudaMemcpyHostToDevice, st));
+  ensure_dynamic_smem(reinterpret_cast<const void*>(resample_kernel), RS_MAX_SMEM);
+  mark(e, st, "resample", 0, bytes);
+  resample_kernel<<<(unsigned)ctas, RS_THREADS, (size_t)smem, st>>>(e->rs_desc, (int)dev.size(), (int)tab_floats);
   SAB_CUDA(cudaGetLastError());
   SAB_API_END
 }

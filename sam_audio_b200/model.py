@@ -368,6 +368,39 @@ class SAMAudio(torch.nn.Module):
         latent = torch.empty(B * c, T, C2, device=dev, dtype=torch.float32)
         return _capi.blend_windows(win_lat, seq.to(dev), start.to(dev), flags.to(dev), window_ramp(Tw), latent)
 
+    @torch.inference_mode()
+    def resample(self, wav: torch.Tensor, orig_sr: int, new_sr: int) -> torch.Tensor:
+        """Band-limited resampling on the GPU (sab_resample; torchaudio's default sinc_interp_hann design):
+
+            x48 = model.resample(x16, 16000, model.sample_rate)     # bring a tensor to the codec's rate ...
+            out = model.separate(processor(descriptions=["dog barking"], audios=[x48[None]]).to("cuda"))
+            y16 = model.resample(out.target[0], model.sample_rate, 16000)   # ... and the result back
+
+        wav: fp32 [S] or [N, S] (rows are separate signals) on the model's device; one side of the pair must be the
+        model's rate, and rates are integers in [8000, 192000] Hz.  Returns [S'] or [N, S'] with S' = ceil(new * S /
+        orig) (gcd-reduced), every row in one launch; wav itself when orig_sr == new_sr."""
+        from .resample import check_rate, resampled_length
+        orig, new = check_rate(orig_sr, "orig_sr"), check_rate(new_sr, "new_sr")
+        if self.sample_rate not in (orig, new):
+            raise ValueError(f"resampling {orig} -> {new} Hz: one side must be the model's rate ({self.sample_rate} Hz)")
+        if not isinstance(wav, torch.Tensor) or wav.dim() not in (1, 2) or wav.shape[-1] < 1:
+            raise ValueError(f"resample() takes [S] or [N, S] samples with S >= 1, got "
+                             f"{tuple(wav.shape) if isinstance(wav, torch.Tensor) else type(wav).__name__}")
+        if wav.dtype != torch.float32 or wav.device != self._device or self._device.type != "cuda":
+            raise ValueError(f"resample() takes fp32 samples on the model's CUDA device ({self._device}), got "
+                             f"{wav.dtype} on {wav.device}")
+        if orig == new:
+            return wav
+        rows = wav.reshape(-1, wav.shape[-1]).contiguous()
+        N, S = rows.shape
+        S2 = resampled_length(S, orig, new)
+        out = torch.empty(N, S2, device=wav.device, dtype=torch.float32)
+        segs = [dict(orig_rate=orig, new_rate=new, in_=rows[i].data_ptr(), in_count=S, length=S,
+                     out=out[i].data_ptr(), out_first=0, out_count=S2) for i in range(N)]
+        with torch.cuda.device(wav.device):
+            self._ensure_engine().resample(segs)
+        return out if wav.dim() == 2 else out[0]
+
     def _stream_args(self, window_seconds: float, ode_opt: Dict[str, Any], reranking_candidates: int, anchors,
                      masked_video):
         """(W, n_steps, method) of a stream, after the checks stream() and stream_group() share."""
@@ -388,13 +421,18 @@ class SAMAudio(torch.nn.Module):
 
     def stream(self, description: str, window_seconds: float = 10.0, seed: int = 0,
                ode_opt: Dict[str, Any] = DFLT_ODE_OPT, reranking_candidates: int = 1, anchors=None,
-               masked_video=None):
+               masked_video=None, sample_rate: Optional[int] = None):
         """Separation of audio that arrives in chunks (sam_audio_b200.stream, DESIGN.md section 3):
 
-            s = model.stream(description="man speaking")
-            for chunk in source:          # [S] or [1, S] float samples at the model's rate, any S >= 1
-                out = s.push(chunk)       # out.target / out.residual: the samples that became final
+            s = model.stream(description="man speaking", sample_rate=16000)
+            for chunk in source:          # [S], [1, S] or [C, S] (C <= 8) float samples at sample_rate, any S >= 1
+                out = s.push(chunk)       # out.target / out.residual: the samples that became final, at sample_rate
             tail = s.flush()              # the rest; the stream is closed afterwards
+
+        sample_rate: an integer in [8000, 192000] Hz (None: the model's rate).  Channels are averaged.  At another rate
+        the stream runs at the model's rate between two resamplers, and its output equals, bit for bit,
+        resample(out, model rate, sample_rate) of the model-rate stream pushed resample(channel mean, sample_rate, model
+        rate), whatever the chunking.
 
         The stream is solved as windows of W = round(window_seconds * 25) latent frames, 8 <= W <= max_positions; the
         default 10 s keeps the DiT on its short-sequence attention (T <= 256).  Text prompts with one candidate only.
@@ -404,7 +442,11 @@ class SAMAudio(torch.nn.Module):
         W, n_steps, method = self._stream_args(window_seconds, ode_opt, reranking_candidates, anchors, masked_video)
         if not isinstance(description, str):
             raise TypeError("a stream separates one source: description must be one string")
-        return StreamGroup(self, W, n_steps, method, resident_plans=False).open(description, seed=int(seed))
+        if sample_rate is not None:
+            from .resample import check_rate
+            check_rate(sample_rate)
+        return StreamGroup(self, W, n_steps, method, resident_plans=False).open(description, seed=int(seed),
+                                                                                 sample_rate=sample_rate)
 
     def stream_group(self, window_seconds: float = 10.0, ode_opt: Dict[str, Any] = DFLT_ODE_OPT,
                      reranking_candidates: int = 1, anchors=None, masked_video=None):
@@ -412,6 +454,7 @@ class SAMAudio(torch.nn.Module):
 
             group = model.stream_group(window_seconds=10.0)
             a = group.open("man speaking", seed=0)      # a stream, with push / flush as from stream()
+            c = group.open("rain", sample_rate=16000)    # ... at its own rate and channel count
             b = group.open("dog barking", seed=7)
             outs = group.push({a: chunk_a, b: chunk_b})  # one tick -> {stream: StreamOutput}
             tails = group.flush([a, b])                  # ends and closes them (a.flush() alone works too)

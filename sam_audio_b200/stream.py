@@ -24,8 +24,16 @@ its call, so a stream's output is bit-identical whatever the other streams of it
 The noise of frame t is row t % H of block t // H, drawn from a generator seeded by (seed, block): overlapping windows
 start from the same noise rows, and nothing depends on how the input was chunked.  Device memory stays bounded by the
 window length, whatever the stream's length: two windows of latents, about W plus two halos of samples and features,
-and the engine's resident plans.  PyTorch only allocates, slices and concatenates here; the arithmetic runs in
-libsamaudio_b200.so.
+and the engine's resident plans.
+
+A stream at another rate, or with several channels, is this stream at the codec's rate with a resampler in front of it
+and one behind it (sab_resample, sam_audio_b200.resample).  Ingest turns the pushed samples into the codec-rate samples
+whose taps have all arrived (the channel mean is taken as the kernel loads them); output resamples the codec-rate
+samples that became final into the stream's rate, emitting a sample once all its taps are final.  At flush() both sides
+know their lengths and apply the zero fill at the end.  In a tick every stream's ingest is one sab_resample call before
+the encode and every stream's output one call after the decode.  Each resampler holds at most K samples plus one push
+(K = its table's taps).  A mono stream at the codec's rate has neither.  PyTorch only allocates, slices and
+concatenates here; the arithmetic runs in libsamaudio_b200.so.
 """
 from __future__ import annotations
 
@@ -37,6 +45,7 @@ from typing import Dict, Iterable, List, Mapping
 import torch
 
 from . import _capi
+from .resample import check_rate, first_tap, outputs_ready, taps
 from .windows import (stream_bucket, stream_emit_end, stream_final_frames, stream_flush_rows,
                       stream_frames_available, stream_group_capacity, stream_hop, stream_tick_groups, stream_window_starts,
                       stream_windows_ready, window_ramp, window_rows_budget)
@@ -86,12 +95,75 @@ def check_tick(group, streams: List) -> None:
         seen.add(id(s))
 
 
-def _samples(chunk: torch.Tensor) -> torch.Tensor:
-    if chunk.dim() == 2 and chunk.shape[0] == 1:
-        chunk = chunk[0]
-    if chunk.dim() != 1 or chunk.numel() < 1:
-        raise ValueError(f"push() takes [S] or [1, S] samples with S >= 1, got shape {tuple(chunk.shape)}")
+MAX_CHANNELS = 8
+
+
+def _samples(chunk: torch.Tensor, channels=None) -> torch.Tensor:
+    """A pushed chunk as [C, S]: [S], [1, S] or [C, S] with 1 <= C <= 8 and S >= 1, and C equal to the channels of the
+    stream's earlier pushes (`channels`, None before the first)."""
+    if not isinstance(chunk, torch.Tensor):
+        raise TypeError(f"push() takes a tensor of samples, got {type(chunk).__name__}")
+    if chunk.dim() == 1:
+        chunk = chunk[None]
+    if chunk.dim() != 2 or chunk.shape[1] < 1 or not 1 <= chunk.shape[0] <= MAX_CHANNELS:
+        raise ValueError(f"push() takes [S], [1, S] or [C, S] samples with 1 <= C <= {MAX_CHANNELS} and S >= 1, got "
+                         f"shape {tuple(chunk.shape)}")
+    if channels is not None and chunk.shape[0] != channels:
+        raise ValueError(f"the stream has {channels} channel(s) (its first push); got a chunk of {chunk.shape[0]}")
     return chunk
+
+
+class _Resampler:
+    """One rate conversion of a stream: the input samples that later outputs still read ([rows, held], inputs
+    [first, received)), and the outputs [0, produced) made so far.  mean=True: the rows are channels of one signal and
+    the output is their mean resampled; mean=False: each row is a signal of its own.  Holds at most K samples plus one
+    push per row."""
+
+    def __init__(self, orig: int, new: int, rows: int, mean: bool, device):
+        self.orig, self.new, self.rows, self.mean = orig, new, rows, mean
+        self.K = taps(orig, new)[0]
+        self.device = device
+        self._buf = self._spare = None
+        self.first = self.received = self.produced = 0
+
+    def append(self, x: torch.Tensor):
+        held, S = self.received - self.first, x.shape[1]
+        if self._buf is None or held + S > self._buf.shape[1]:
+            buf = torch.empty(self.rows, 2 * (held + S) + self.K, device=self.device, dtype=torch.float32)
+            if held:
+                buf[:, :held].copy_(self._buf[:, :held])
+            self._buf, self._spare = buf, torch.empty_like(buf)
+        self._buf[:, held:held + S].copy_(x)
+        self.received += S
+
+    def take(self, flushed: bool):
+        """(segments, out): the sab_resample segments of the outputs that became computable (all of them once flushed,
+        when the input's length is known) and their output tensor [1 if mean else rows, count]."""
+        q0 = self.produced
+        q1 = max(q0, outputs_ready(self.received, self.orig, self.new, self.received if flushed else None))
+        out = torch.empty(1 if self.mean else self.rows, q1 - q0, device=self.device, dtype=torch.float32)
+        segs = []
+        if q1 > q0:
+            seg = dict(orig_rate=self.orig, new_rate=self.new, in_first=self.first,
+                       in_count=self.received - self.first, length=self.received if flushed else -1, out_first=q0,
+                       out_count=q1 - q0)
+            if self.mean:
+                segs.append(dict(seg, channels=self.rows, in_=self._buf.data_ptr(),
+                                 in_channel_stride=self._buf.shape[1], out=out.data_ptr()))
+            else:
+                segs += [dict(seg, in_=self._buf[r].data_ptr(), out=out[r].data_ptr()) for r in range(self.rows)]
+        self.produced = q1
+        return segs, out
+
+    def trim(self):
+        """Drop the inputs no later output reads (after the launch that read them is enqueued)."""
+        keep0 = min(self.received, max(0, first_tap(self.produced, self.orig, self.new)))
+        if keep0 <= self.first:
+            return
+        a, b = keep0 - self.first, self.received - self.first
+        self._spare[:, :b - a].copy_(self._buf[:, a:b])
+        self._buf, self._spare = self._spare, self._buf
+        self.first = keep0
 
 
 class SeparationStream:
@@ -99,9 +171,14 @@ class SeparationStream:
     final, ``flush`` the rest, and the concatenation of everything returned is ceil(n / hop) * hop samples for n samples
     pushed.  ``push`` and ``flush`` are ticks of the stream's group with this stream alone."""
 
-    def __init__(self, group: "StreamGroup", description: str, seed: int):
+    def __init__(self, group: "StreamGroup", description: str, seed: int, sample_rate: int):
         self.group = group
         self.model = group.model
+        self.sample_rate = sample_rate                         # of push() and of the outputs
+        self.channels = None                                   # of push(), fixed by the first
+        self._ingest = None                                    # resampler to the codec's rate (set by the first push)
+        sr = self.model.sample_rate
+        self._emit = None if sample_rate == sr else _Resampler(sr, sample_rate, 2, False, group.device)
         self.W, self.O, self.H, self.hop, self.C = group.W, group.O, group.H, group.hop, group.C
         self.seed = seed
         self.device = group.device
@@ -128,7 +205,8 @@ class SeparationStream:
 
     # ------------------------------------------------------------------ public
     def push(self, chunk: torch.Tensor) -> StreamOutput:
-        """Append samples ([S] or [1, S], S >= 1) and return the samples that became final."""
+        """Append samples ([S], [1, S] or [C, S] with 1 <= C <= 8, S >= 1, at the stream's rate) and return the samples
+        that became final, at the stream's rate."""
         return self.group.push({self: chunk})[self]
 
     def flush(self) -> StreamOutput:
@@ -173,6 +251,14 @@ class SeparationStream:
 
     def _release(self):
         self._buf = self._spare = self._feat = self._lat = self._prev = None
+        self._ingest = self._emit = None
+
+    def _set_channels(self, C: int):
+        if self.channels is None:
+            self.channels = C
+            sr = self.model.sample_rate
+            if self.sample_rate != sr or C > 1:
+                self._ingest = _Resampler(self.sample_rate, sr, C, True, self.device)
 
     def _output(self, pieces: List[torch.Tensor]) -> StreamOutput:
         if not pieces:
@@ -215,33 +301,39 @@ class StreamGroup:
             self._finalizer.atexit = False
 
     # ------------------------------------------------------------------ public
-    def open(self, description: str, seed: int = 0) -> SeparationStream:
-        """A new stream of the group with its own prompt and noise seed."""
+    def open(self, description: str, seed: int = 0, sample_rate=None) -> SeparationStream:
+        """A new stream of the group with its own prompt and noise seed.  sample_rate: of its pushes and outputs (an
+        integer in [8000, 192000] Hz; None: the model's rate)."""
         if self.closed:
             raise RuntimeError("the stream group is closed")
         if not isinstance(description, str):
             raise TypeError("a stream separates one source: description must be one string")
-        s = SeparationStream(self, description, int(seed))
+        sr = self.model.sample_rate if sample_rate is None else check_rate(sample_rate)
+        s = SeparationStream(self, description, int(seed), sr)
         self.L = max(self.L, s.n_tokens)
         self.streams.append(s)
         return s
 
     @torch.inference_mode()
     def push(self, chunks: Mapping[SeparationStream, torch.Tensor]) -> Dict[SeparationStream, StreamOutput]:
-        """One tick: append each stream's samples ([S] or [1, S], S >= 1) and return, per stream, the samples that
-        became final."""
+        """One tick: append each stream's samples ([S], [1, S] or [C, S], S >= 1, at its rate) and return, per stream,
+        the samples that became final, at its rate."""
         streams = list(chunks)
         check_tick(self, streams)
-        xs = [_samples(chunks[s]).to(device=self.device, dtype=torch.float32) for s in streams]
+        xs = [_samples(chunks[s], s.channels).to(device=self.device, dtype=torch.float32) for s in streams]
         with torch.cuda.device(self.device):
+            for s, x in zip(streams, xs):
+                s._set_channels(x.shape[0])
+            ingested = self._resample_in(streams, xs, flushed=False)
             due = []
             for s, x in zip(streams, xs):
-                s._append(x)
+                s._append(ingested.get(s, x[0]))
                 avail = stream_frames_available(s.n_samples, self.hop, self.halo_enc)
                 due.append((s, s.windows_solved, stream_windows_ready(avail, self.W)))
             out = self._tick(due, flushed=False)
             for s in streams:
                 s._trim_samples()
+            out = self._resample_out(out, flushed=False)
         return out
 
     @torch.inference_mode()
@@ -249,15 +341,20 @@ class StreamGroup:
         """One tick that ends the given streams: each returns every sample not returned yet and is closed."""
         streams = list(streams)
         check_tick(self, streams)
-        live = [s for s in streams if s.n_samples > 0]
         try:
             with torch.cuda.device(self.device):
+                # the ingest's zero fill at the end: the codec-rate stream gets the rest of its samples first
+                for s, x in self._resample_in(streams, [None] * len(streams), flushed=True).items():
+                    if x.numel():
+                        s._append(x)
+                live = [s for s in streams if s.n_samples > 0]
                 for s in live:
                     s.n_final = -(-s.n_samples // self.hop)
                 out = self._tick([(s, s.windows_solved, len(stream_window_starts(s.n_final, self.W))) for s in live],
                                  flushed=True)
                 for s in streams:
                     out.setdefault(s, s._output([]))
+                out = self._resample_out(out, flushed=True)
         finally:
             # a stream is ended whether or not its last tick succeeded: a failed flush leaves no half-advanced stream
             # in the group, so close() still works and gives the engine back its residency
@@ -302,6 +399,44 @@ class StreamGroup:
 
     def __exit__(self, *exc):
         self.close()
+
+    # ------------------------------------------------------------------ rate conversion
+    def _resample_in(self, streams, xs, flushed: bool) -> Dict[SeparationStream, torch.Tensor]:
+        """Ingest of a tick, one sab_resample call for every stream that has a resampler in front: the codec-rate
+        samples that became computable (all the rest at flush()), per stream.  xs: the pushed [C, S] (None at flush)."""
+        segs, outs = [], {}
+        for s, x in zip(streams, xs):
+            r = s._ingest
+            if r is None:
+                continue
+            if x is not None:
+                r.append(x)
+            sg, out = r.take(flushed)
+            segs += sg
+            outs[s] = out[0]
+        self.model._ensure_engine().resample(segs)
+        for s in outs:
+            s._ingest.trim()
+        return outs
+
+    def _resample_out(self, out: Dict[SeparationStream, StreamOutput], flushed: bool) -> Dict[SeparationStream,
+                                                                                             StreamOutput]:
+        """Output of a tick, one sab_resample call for every stream that has a resampler behind: the codec-rate samples
+        that became final are appended to it, and the stream-rate samples whose taps are all final are returned."""
+        segs, ys = [], {}
+        for s, o in out.items():
+            r = s._emit
+            if r is None:
+                continue
+            if o.target.numel():
+                r.append(torch.stack([o.target, o.residual]))
+            sg, ys[s] = r.take(flushed)
+            segs += sg
+        self.model._ensure_engine().resample(segs)
+        for s, y in ys.items():
+            s._emit.trim()
+            out[s] = StreamOutput(target=y[0], residual=y[1])
+        return out
 
     # ------------------------------------------------------------------ the tick
     def _tick(self, due, flushed: bool) -> Dict[SeparationStream, StreamOutput]:

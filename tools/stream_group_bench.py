@@ -12,9 +12,12 @@ planned and captured), over --ticks timed ticks, with the card's name and power 
   - group.close() of all S streams in one flush tick: its wall time and the plans it built per stream that left;
 and the same S streams each run alone through SAMAudio.stream(), pushed round-robin (one round = one push per stream;
 skipped once a smaller S already missed real time there, or with --no-solo).  The real-time capacity is the largest S
-whose 90th-percentile tick (round) is below the push interval.  Prints one JSON line at the end.  Fails without a GPU.
+whose 90th-percentile tick (round) is below the push interval.  With --sample-rate every stream runs at that rate
+(SAMAudio.stream(sample_rate=...)): each tick then adds one resampling launch in front of the encode and one after the
+decode.  Prints one JSON line at the end.  Fails without a GPU.
 
     python tools/stream_group_bench.py [--streams 16,32,64,96,128] [--ticks 30] [--warmup 20] [--solo-ticks 20]
+                                       [--sample-rate 16000]
 """
 import argparse
 import json
@@ -42,17 +45,19 @@ def run(m, S, args, solo: bool):
     sr, hop = m.cfg.audio_codec.sample_rate, m.cfg.audio_codec.hop_length
     W = int(round(args.window_seconds * sr / hop))
     H = stream_hop(W)
-    push = int(round(args.push_seconds * sr))
+    rate = args.sample_rate or sr
+    push = int(round(args.push_seconds * rate))
     n_ticks = args.warmup + (args.solo_ticks if solo else args.ticks)
     gen = torch.Generator(device="cuda").manual_seed(S)
-    pre = [(i * H * hop) // S for i in range(S)]
+    pre = [(i * H * hop * rate // sr) // S for i in range(S)]
     wav = 0.1 * torch.randn(S, max(pre) + n_ticks * push, generator=gen, device="cuda")
     eng = m._ensure_engine()
     group = None if solo else m.stream_group(window_seconds=args.window_seconds)
     if solo:
-        streams = [m.stream(PROMPTS[i % len(PROMPTS)], window_seconds=args.window_seconds, seed=i) for i in range(S)]
+        streams = [m.stream(PROMPTS[i % len(PROMPTS)], window_seconds=args.window_seconds, seed=i,
+                            sample_rate=args.sample_rate) for i in range(S)]
     else:
-        streams = [group.open(PROMPTS[i % len(PROMPTS)], seed=i) for i in range(S)]
+        streams = [group.open(PROMPTS[i % len(PROMPTS)], seed=i, sample_rate=args.sample_rate) for i in range(S)]
     for i, s in enumerate(streams):
         if pre[i]:
             s.push(wav[i, :pre[i]])
@@ -119,6 +124,7 @@ def main():
     ap.add_argument("--no-solo", action="store_true")
     ap.add_argument("--push-seconds", type=float, default=1.0)
     ap.add_argument("--window-seconds", type=float, default=10.0)
+    ap.add_argument("--sample-rate", type=int, default=None, help="of every stream (default: the model's rate)")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "stream_group_bench needs a GPU"
     import __graft_entry__ as g
@@ -165,7 +171,8 @@ def main():
     cap = max([S for S, v in sweep.items() if v["tick_ms"]["p90"] < interval_ms], default=0)
     solo_cap = max([S for S, v in solo_sweep.items() if v["round_ms"]["p90"] < interval_ms], default=0)
     res = {"device": name, "power_limit": limit, "model": args.model, "window_frames": W, "hop_frames": stream_hop(W),
-           "push_seconds": args.push_seconds, "ticks": args.ticks, "warmup": args.warmup,
+           "sample_rate": args.sample_rate or cfg.audio_codec.sample_rate, "push_seconds": args.push_seconds,
+           "ticks": args.ticks, "warmup": args.warmup,
            "realtime_capacity_streams": cap, "solo_realtime_capacity_streams": solo_cap,
            "solo_capacity_bounded_by_sweep": bool(solo_sweep) and max(solo_sweep) == solo_cap,
            "group": {str(k): v for k, v in sweep.items()}, "solo": {str(k): v for k, v in solo_sweep.items()}}
