@@ -468,7 +468,19 @@ class SAMAudio(torch.nn.Module):
         one DiT plan per bucket of window counts it has used resident (and the codec plans of those buckets), so ticks
         of varying size do not re-plan; close() restores the default residency, and so does collecting a group dropped
         without close().  A flush tick reuses the buckets of earlier ticks, so ending many streams at once plans no
-        larger DiT bucket beside them."""
+        larger DiT bucket beside them.
+
+        Offline jobs take the ticks' filler slots (the spare slots of each bucket, otherwise repeated live items):
+
+            job = group.submit(wav, "dog barking", seed=3, sample_rate=16000)   # a whole recording, [S] or [C, S]
+            group.drain([job])                   # ticks of jobs only, at buckets the group uses; close() drains too
+            out = job.result()                   # == model.stream(...) with wav pushed once and flushed, bit for bit
+
+        A job is cut into codec tiles of the steady slice lengths, so in push ticks it adds no planned call, changes no
+        call's item count and builds no plan; live streams keep their bits.  The exception is a job prompt longer than
+        every prompt of the group: like open(), it raises the group's text length, and the next tick re-plans every
+        bucket at it.  submit() copies the recording.  Jobs run first in, first out; job.cancel()
+        frees one, and a group collected without close() cancels its jobs."""
         from .stream import StreamGroup
         W, n_steps, method = self._stream_args(window_seconds, ode_opt, reranking_candidates, anchors, masked_video)
         return StreamGroup(self, W, n_steps, method, resident_plans=True)

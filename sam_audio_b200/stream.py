@@ -26,6 +26,9 @@ start from the same noise rows, and nothing depends on how the input was chunked
 window length, whatever the stream's length: two windows of latents, about W plus two halos of samples and features,
 and the engine's resident plans.
 
+A job (``StreamGroup.submit``) is a stream whose whole input is known: it runs in the filler slots of push ticks, with
+its encodes and decodes cut into tiles of the steady slice lengths so that it only joins calls the tick makes anyway.
+
 A stream at another rate, or with several channels, is this stream at the codec's rate with a resampler in front of it
 and one behind it (sab_resample, sam_audio_b200.resample).  Ingest turns the pushed samples into the codec-rate samples
 whose taps have all arrived (the channel mean is taken as the kernel loads them); output resamples the codec-rate
@@ -45,10 +48,11 @@ from typing import Dict, Iterable, List, Mapping
 import torch
 
 from . import _capi
-from .resample import check_rate, first_tap, outputs_ready, taps
-from .windows import (stream_bucket, stream_emit_end, stream_final_frames, stream_flush_rows,
-                      stream_frames_available, stream_group_capacity, stream_hop, stream_tick_groups, stream_window_starts,
-                      stream_windows_ready, window_ramp, window_rows_budget)
+from .resample import check_rate, first_tap, outputs_ready, resampled_length, taps
+from .windows import (TickWindows, stream_bucket, stream_drain_bucket, stream_emit_end, stream_final_frames,
+                      stream_flush_rows, stream_frames_available, stream_group_capacity, stream_hop, stream_job_admit,
+                      stream_job_min_frames, stream_job_slots, stream_steady_slices, stream_tick_groups, stream_tiles,
+                      stream_window_starts, stream_windows_ready, window_ramp, window_rows_budget)
 
 _NULL_ANCHOR_IDS = (0, 3)   # the processor's ids of a clip without anchors: <null>, <pad> (processor.py)
 
@@ -98,15 +102,15 @@ def check_tick(group, streams: List) -> None:
 MAX_CHANNELS = 8
 
 
-def _samples(chunk: torch.Tensor, channels=None) -> torch.Tensor:
+def _samples(chunk: torch.Tensor, channels=None, what: str = "push()") -> torch.Tensor:
     """A pushed chunk as [C, S]: [S], [1, S] or [C, S] with 1 <= C <= 8 and S >= 1, and C equal to the channels of the
-    stream's earlier pushes (`channels`, None before the first)."""
+    stream's earlier pushes (`channels`, None before the first).  `what` names the call in the messages."""
     if not isinstance(chunk, torch.Tensor):
-        raise TypeError(f"push() takes a tensor of samples, got {type(chunk).__name__}")
+        raise TypeError(f"{what} takes a tensor of samples, got {type(chunk).__name__}")
     if chunk.dim() == 1:
         chunk = chunk[None]
     if chunk.dim() != 2 or chunk.shape[1] < 1 or not 1 <= chunk.shape[0] <= MAX_CHANNELS:
-        raise ValueError(f"push() takes [S], [1, S] or [C, S] samples with 1 <= C <= {MAX_CHANNELS} and S >= 1, got "
+        raise ValueError(f"{what} takes [S], [1, S] or [C, S] samples with 1 <= C <= {MAX_CHANNELS} and S >= 1, got "
                          f"shape {tuple(chunk.shape)}")
     if channels is not None and chunk.shape[0] != channels:
         raise ValueError(f"the stream has {channels} channel(s) (its first push); got a chunk of {chunk.shape[0]}")
@@ -249,6 +253,11 @@ class SeparationStream:
         f[:n], m[:n] = self._text[0], self._text_mask[0]
         return f, m
 
+    def _ends_at(self, kb: int) -> bool:
+        """Window kb - 1 is the stream's last, which carries its end (WIN_LAST, the pad mask past n_final): known once
+        the stream's length is, at flush() (a job: from the start)."""
+        return self.n_final is not None and kb == len(stream_window_starts(self.n_final, self.W))
+
     def _release(self):
         self._buf = self._spare = self._feat = self._lat = self._prev = None
         self._ingest = self._emit = None
@@ -266,6 +275,108 @@ class SeparationStream:
             return StreamOutput(target=e, residual=e.clone())
         w = pieces[0] if len(pieces) == 1 else torch.cat(pieces, 1)
         return StreamOutput(target=w[0], residual=w[1])
+
+
+class SeparationJob:
+    """Returned by ``StreamGroup.submit()``: a whole recording separated in the idle slots of the group's ticks.  It is
+    the stream ``model.stream(description, window_seconds, seed, sample_rate)`` would be with the recording pushed once
+    and flushed: the same windows, noise, blend and resamplers, so ``result()`` equals that stream's concatenated output
+    bit for bit.  Its encodes and decodes are cut into tiles of the steady slice lengths (windows.stream_tiles).
+
+    It holds the recording at the codec's rate (until it is encoded), the output at the codec's rate as it is decoded
+    (at its own rate once done), and a stream's per-window state; features and latents are kept from the next window's
+    and the next decode tile's first frame on.  All of it is bounded by its own length."""
+
+    _text_at = SeparationStream._text_at
+    _ends_at = SeparationStream._ends_at
+
+    def __init__(self, group: "StreamGroup", description: str, seed: int, sample_rate: int, wav: torch.Tensor):
+        self._group = weakref.ref(group)      # the group's finalizer cancels its jobs, so a job must not keep it alive
+        self.model = group.model
+        self.sample_rate = sample_rate
+        self.W, self.O, self.H, self.hop, self.C = group.W, group.O, group.H, group.hop, group.C
+        self.seed = seed
+        self.device = group.device
+        with torch.cuda.device(self.device):
+            tf, tm = self.model.text_encoder([description])
+        self._text = tf.to(self.device, torch.float32).contiguous()
+        self._text_mask = tm.to(self.device).contiguous()
+        self.n_tokens = self._text.shape[1]
+        sr = self.model.sample_rate
+        with torch.cuda.device(self.device):
+            if sample_rate != sr or wav.shape[0] > 1:        # the stream's ingest, with the whole length known
+                x = wav.to(device=self.device, dtype=torch.float32).contiguous()
+                S = x.shape[1]
+                x48 = torch.empty(1, resampled_length(S, sample_rate, sr), device=self.device, dtype=torch.float32)
+                self.model._ensure_engine().resample([dict(
+                    orig_rate=sample_rate, new_rate=sr, channels=x.shape[0], in_=x.data_ptr(), in_channel_stride=S,
+                    in_first=0, in_count=S, length=S, out=x48.data_ptr(), out_first=0, out_count=x48.shape[1])])
+            else:
+                # a copy, as push() makes one: the tiles read the recording over later ticks, and the caller may reuse
+                # its tensor as soon as submit() returns
+                x48 = wav.to(device=self.device, dtype=torch.float32, copy=True).contiguous()
+            self._wav = self.model._pad(x48)[0]               # reflect-padded to n_final frames, as flush() pads
+        self.n_samples = x48.shape[1]
+        self._init_schedule(-(-self.n_samples // self.hop), group.halo_enc, group.halo_dec)
+        self._feat = torch.empty(0, self.C, device=self.device)
+        self._prev = None
+        self._lat = torch.empty(0, self.C, device=self.device)
+        self._out = torch.empty(2, self.n_final * self.hop, device=self.device, dtype=torch.float32)
+        self._result = None
+        self.done = self.cancelled = False
+
+    def _init_schedule(self, n_final: int, halo_enc: int, halo_dec: int):
+        """The job's tile plans and progress counters for a recording of n_final frames (host state only)."""
+        self.n_final = n_final
+        self._enc_len, self._dec_len = le, ld = stream_steady_slices(self.W, halo_enc, halo_dec)
+        self._enc_tiles = stream_tiles(n_final, le, halo_enc)
+        self._dec_tiles = stream_tiles(n_final, ld, halo_dec)
+        self._enc_next = self._dec_next = 0                   # tiles done
+        self.windows_total = len(stream_window_starts(n_final, self.W))
+        self.windows_solved = 0
+        self._enc_end = self._feat0 = 0                       # features [0, _enc_end) encoded, [_feat0, ...) kept
+        self.final_frames = self._lat0 = 0                    # latents [0, final_frames) final, [_lat0, ...) kept
+
+    # ------------------------------------------------------------------ public
+    def result(self) -> StreamOutput:
+        """The separated recording at the job's rate: the concatenated target and residual of the stream above."""
+        if self.cancelled:
+            raise RuntimeError("the job was cancelled")
+        if not self.done:
+            raise RuntimeError(f"the job is not done ({self.windows_solved} of {self.windows_total} windows solved): "
+                               "its group runs it in idle slots of push ticks; group.drain() finishes it")
+        return self._result
+
+    def cancel(self) -> None:
+        """Stop the job and free its device memory (its result too, if it is done)."""
+        self.cancelled = True
+        self._release()
+        self._result = None
+        g = self._group()
+        if g is not None and self in g._jobs:
+            g._jobs.remove(self)
+
+    # ------------------------------------------------------------------ what the next calls can take
+    def _encode_offer(self) -> int:
+        return len(self._enc_tiles) - self._enc_next
+
+    def _solve_offer(self) -> int:
+        """Windows ready to solve: their features are encoded (the last one's once the whole recording is)."""
+        if self._enc_next == len(self._enc_tiles):
+            return self.windows_total - self.windows_solved
+        return max(0, min(self.windows_total, stream_windows_ready(self._enc_end, self.W)) - self.windows_solved)
+
+    def _decode_offer(self) -> int:
+        """Decode tiles whose latent frames are all final."""
+        n = 0
+        for start, _, _ in self._dec_tiles[self._dec_next:]:
+            if start + self._dec_len > self.final_frames:
+                break
+            n += 1
+        return n
+
+    def _release(self):
+        self._wav = self._feat = self._lat = self._prev = self._out = self._text = self._text_mask = None
 
 
 class StreamGroup:
@@ -287,6 +398,7 @@ class StreamGroup:
         # that carries the stream's end (WIN_LAST)
         assert self.halo_enc >= 1
         self.capacity = stream_group_capacity(W, window_rows_budget())
+        self._steady = stream_steady_slices(W, self.halo_enc, self.halo_dec)   # frames of steady encode/decode slices
         self.L = 0                      # text tokens of every window: the longest prompt opened in the group so far
         self.streams: List[SeparationStream] = []
         self._ids = torch.tensor([_NULL_ANCHOR_IDS], dtype=torch.long, device=self.device)
@@ -294,10 +406,11 @@ class StreamGroup:
         self._holds_limits = resident_plans
         self._buckets_used = set()     # item counts of the planned calls of push ticks (the residency follows them)
         self._solve_buckets = set()    # ... of their solves: the DiT plans a flush tick reuses
+        self._jobs: List[SeparationJob] = []   # submitted and not done, first in first out
         if resident_plans:
-            # a group dropped without close() gives the residency back when it is collected
+            # a group dropped without close() cancels its jobs and gives the residency back when it is collected
             self._limits_key = object()
-            self._finalizer = weakref.finalize(self, model._hold_plan_limits, self._limits_key, None)
+            self._finalizer = weakref.finalize(self, _drop_group, model._hold_plan_limits, self._limits_key, self._jobs)
             self._finalizer.atexit = False
 
     # ------------------------------------------------------------------ public
@@ -313,6 +426,44 @@ class StreamGroup:
         self.L = max(self.L, s.n_tokens)
         self.streams.append(s)
         return s
+
+    @torch.inference_mode()
+    def submit(self, wav: torch.Tensor, description: str, seed: int = 0, sample_rate=None) -> SeparationJob:
+        """Queue a whole recording ([S], [1, S] or [C, S] with C <= 8, at sample_rate) to be separated in the idle slots
+        of the group's ticks; see SeparationJob.  sample_rate and the prompt are as for open() (the prompt counts
+        toward the group's text length: a prompt longer than every earlier one makes the next tick re-plan its buckets
+        at the new length, as open() does).  The recording is copied, so the caller may reuse its tensor at once.  It
+        must be long enough to be cut into codec tiles of the steady slice lengths (stream_job_min_frames)."""
+        if self.closed:
+            raise RuntimeError("the stream group is closed")
+        if not isinstance(description, str):
+            raise TypeError("a job separates one source: description must be one string")
+        sr = self.model.sample_rate if sample_rate is None else check_rate(sample_rate)
+        x = _samples(wav, what="submit()")
+        n48 = x.shape[1] if sr == self.model.sample_rate else resampled_length(x.shape[1], sr, self.model.sample_rate)
+        need = stream_job_min_frames(self.W, self.halo_enc, self.halo_dec)
+        if -(-n48 // self.hop) < need:
+            raise ValueError(f"a job of {x.shape[1] / sr:.3f} s is too short: a stream group's jobs need at least "
+                             f"{need * self.hop / self.model.sample_rate:.3f} s ({need} latent frames) at this window "
+                             "length; separate() or stream() take shorter recordings")
+        job = SeparationJob(self, description, int(seed), sr, x)
+        self.L = max(self.L, job.n_tokens)
+        self._jobs.append(job)
+        return job
+
+    @torch.inference_mode()
+    def drain(self, jobs=None) -> None:
+        """Run ticks that hold only jobs until the given jobs (default: all) are done.  Jobs are served first in, first
+        out, so the jobs submitted before them finish too.  Each planned call runs at a solve bucket the group has
+        already used (bucket 1 if it has never ticked), and these ticks are the only ones in which a job may build a
+        plan."""
+        want = list(self._jobs) if jobs is None else list(jobs)
+        for j in want:
+            if not isinstance(j, SeparationJob) or j._group() is not self:
+                raise ValueError("drain() takes jobs submitted to this group")
+        with torch.cuda.device(self.device):
+            while any(not (j.done or j.cancelled) for j in want):
+                self._tick([], flushed=False, drain=True)
 
     @torch.inference_mode()
     def push(self, chunks: Mapping[SeparationStream, torch.Tensor]) -> Dict[SeparationStream, StreamOutput]:
@@ -365,11 +516,16 @@ class StreamGroup:
         return out
 
     def close(self) -> Dict[SeparationStream, StreamOutput]:
-        """Flush every open stream, close the group and give the engine back its default plan residency."""
+        """Flush every open stream, finish the jobs left (drain()), close the group and give the engine back its
+        default plan residency.  Jobs still queued when a tick fails are cancelled."""
         self.closed = True
         try:
-            return self.flush(list(self.streams)) if self.streams else {}
+            out = self.flush(list(self.streams)) if self.streams else {}
+            self.drain()
+            return out
         finally:
+            for j in list(self._jobs):
+                j.cancel()
             self._release_limits()
 
     def _release_limits(self):
@@ -439,27 +595,50 @@ class StreamGroup:
         return out
 
     # ------------------------------------------------------------------ the tick
-    def _tick(self, due, flushed: bool) -> Dict[SeparationStream, StreamOutput]:
+    def _tick(self, due, flushed: bool, drain: bool = False) -> Dict[SeparationStream, StreamOutput]:
         """Solve windows [k0, k_end) of every (stream, k0, k_end) in due, group by group: encode, solve, blend and decode
-        what each group makes final."""
+        what each group makes final.  In a push tick the queued jobs take the filler slots of its calls; a drain tick
+        (due empty) holds only jobs, and a flush tick none."""
         pieces: Dict[SeparationStream, List[torch.Tensor]] = {s: [] for s, _, _ in due}
         budget = window_rows_budget()
         if flushed and self._holds_limits:
             budget = stream_flush_rows(budget, self.W, self._solve_buckets)
-        for grp in stream_tick_groups(due, self.W, budget):
-            self._encode(grp, flushed)
-            rows = self._solve(grp, flushed)
-            self._blend(grp, rows, flushed)
-            for s, piece in self._decode(grp, flushed):
+        jobs = [] if flushed else list(self._jobs)
+        for grp in ([[]] if drain else stream_tick_groups(due, self.W, budget)):
+            self._encode(grp, flushed, jobs, drain)
+            rows, job_windows = self._solve(grp, flushed, jobs, drain)
+            if rows is not None:
+                self._blend(grp + job_windows, rows)
+            for s, piece in self._decode(grp, flushed, jobs, drain):
                 pieces[s].append(piece)
+        if jobs:
+            self._finish_jobs(jobs)
         return {s: s._output(p) for s, p in pieces.items()}
 
-    def _encode(self, grp, flushed: bool):
+    def _call_slots(self, n_live: int, flushed: bool, solve: bool, jobs, offer, drain: bool):
+        """(slots, taken) of one planned call with n_live live items: a push tick's call runs at its bucket (_slots) and
+        the jobs take its filler slots, first in first out (stream_job_admit, offer(job) = the job's items ready for
+        it); a drain tick's call runs at a resident solve bucket (stream_drain_bucket), or not at all (slots None)
+        when no job has an item ready.  taken: the job items of the call, per job."""
+        offers = [offer(j) for j in jobs]
+        if drain:
+            if not any(offers):
+                return None, offers
+            size = stream_drain_bucket(sum(offers), self._solve_buckets)
+        else:
+            slots = self._slots(n_live, flushed, solve)
+            if not any(offers):
+                return slots, [0] * len(jobs)
+            size = len(slots)
+        taken = stream_job_admit(offers, size - n_live)
+        return stream_job_slots(n_live, size, sum(taken)), taken
+
+    def _encode(self, grp, flushed: bool, jobs=(), drain: bool = False):
         """Encode the frames the group's windows need: [_enc_end, k * H + W) per window, or up to the stream's end at
         flush().  A slice reads halo_enc frames of samples on each side; at a stream's start it starts at sample 0, at
-        flush() it ends at the (reflect-padded) end of the stream."""
+        flush() it ends at the (reflect-padded) end of the stream.  Jobs' tiles fill the call of steady slices."""
         hop, halo = self.hop, self.halo_enc
-        jobs = []                                              # (stream, samples, first kept row, end row, new end)
+        items = []                                             # (stream, samples, first kept row, end row, new end)
         for w in grp:
             s = w.key
             a = s._enc_end
@@ -474,31 +653,54 @@ class StreamGroup:
                     s1 = f1 + halo
                     wav = s._buf[s0 * hop - s._wav0:s1 * hop - s._wav0]
                 assert wav.numel() == (s1 - s0) * hop
-                jobs.append((s, wav, a - s0, f1 - s0, f1))
+                items.append((s, wav, a - s0, f1 - s0, f1))
                 a = f1
-        feats = [None] * len(jobs)
         by_len = defaultdict(list)
-        for i, j in enumerate(jobs):
+        for i, j in enumerate(items):
             by_len[j[1].numel()].append(i)
+        steady = self._steady[0]
+        if drain:
+            by_len.setdefault(steady * hop, [])                # a drain tick has no live items: make the steady call
+        feats = {}
         eng = self.model._ensure_engine()
         for n, idx in by_len.items():
-            slots = self._slots(len(idx), flushed, solve=False)
-            wav = torch.stack([jobs[idx[i]][1] for i in slots])
+            if n == steady * hop and (jobs or drain):
+                slots, taken = self._call_slots(len(idx), flushed, False, jobs, SeparationJob._encode_offer, drain)
+                if slots is None:
+                    continue
+                for j, t in zip(jobs, taken):
+                    for start, k0, k1 in j._enc_tiles[j._enc_next:j._enc_next + t]:
+                        idx.append(len(items))
+                        items.append((j, j._wav[start * hop:(start + steady) * hop], k0 - start, k1 - start, k1))
+                    j._enc_next += t
+            else:
+                slots = self._slots(len(idx), flushed, solve=False)
+            wav = torch.stack([items[idx[i]][1] for i in slots])
             out = torch.empty(len(slots), n // hop, self.C, device=self.device, dtype=torch.float32)
             eng.encode(wav, out)
             for i, ji in enumerate(idx):
                 feats[ji] = out[i]
-        for (s, _, r0, r1, f1), f in zip(jobs, feats):          # in job order: a stream's slices follow each other
-            s._feat = torch.cat([s._feat, f[r0:r1]])
+        for i, (s, _, r0, r1, f1) in enumerate(items):          # in item order: a stream's slices follow each other
+            s._feat = torch.cat([s._feat, feats[i][r0:r1]])
             s._enc_end = f1
+        for j in jobs:
+            if j._enc_next == len(j._enc_tiles):
+                j._wav = None                                  # encoded: the recording is no longer read
 
-    def _solve(self, grp, flushed: bool) -> torch.Tensor:
-        """Prepare and solve the group's windows as one batch of clips of W frames; returns their latents [n, W, C]."""
+    def _solve(self, grp, flushed: bool, jobs=(), drain: bool = False):
+        """Prepare and solve the group's windows, then the job windows the call takes, as one batch of clips of W frames.
+        Returns their latents [n, W, C] (None when a drain tick has nothing to solve) and the job windows."""
         W, H, C, dev = self.W, self.H, self.C, self.device
+        n_live = sum(w.kb - w.ka for w in grp)
+        slots, taken = self._call_slots(n_live, flushed, True, jobs, SeparationJob._solve_offer, drain)
+        if slots is None:
+            return None, []
+        job_windows = [TickWindows(j, j.windows_solved, j.windows_solved + t, j._ends_at(j.windows_solved + t))
+                       for j, t in zip(jobs, taken) if t]
         feats, texts, masks, pads, aligns, noise = [], [], [], [], [], []
-        for w in grp:
+        for w in grp + job_windows:
             s = w.key
-            n_valid = s.n_final if flushed and w.last else None
+            n_valid = s.n_final if s._ends_at(w.kb) else None
             need = (w.kb - 1) * H + W                          # features of frames [ka * H, need)
             if need > s._enc_end:                              # past the end of the stream: zero, under the pad mask
                 s._feat = torch.cat([s._feat, torch.zeros(need - s._enc_end, C, device=dev)])
@@ -518,16 +720,15 @@ class StreamGroup:
                 aligns.append(align)
                 noise.append(stream_noise(s.seed, k * H, k * H + W, H, C, dev))
         n = len(feats)
-        slots = self._slots(n, flushed, solve=True)
         pick = lambda xs: torch.stack([xs[i] for i in slots])   # noqa: E731
         nb = len(slots)
         self.model._install_conditioning(pick(feats), pick(texts), pick(masks), None, self._ids.expand(nb, -1),
                                          pick(aligns), pick(pads), candidates=1)
         rows = pick(noise)
         self.model._ensure_engine().solve(rows, self.n_steps, rows, self.method)
-        return rows[:n]
+        return rows[:n], job_windows
 
-    def _blend(self, grp, rows: torch.Tensor, flushed: bool):
+    def _blend(self, grp, rows: torch.Tensor):
         """Blend each stream's frames that became final from its previous window and the windows just solved; streams
         that finalise the same number of frames share one sab_blend_windows call (one output sequence each)."""
         W, H, C, dev = self.W, self.H, self.C, self.device
@@ -535,14 +736,14 @@ class StreamGroup:
         i = 0
         for w in grp:
             s = w.key
-            f_new = stream_final_frames(w.kb, W, s.n_final if flushed and w.last else -1)
+            f_new = stream_final_frames(w.kb, W, s.n_final if s._ends_at(w.kb) else -1)
             by_count[f_new - s.final_frames].append((w, rows[i:i + w.kb - w.ka], f_new))
             i += w.kb - w.ka
         for count, members in by_count.items():
             wins, seq, start, flags = [], [], [], []
             for q, (w, solved, _) in enumerate(members):
                 s = w.key
-                last_group = flushed and w.last
+                last_group = s._ends_at(w.kb)
                 ks = list(range(w.ka - (s._prev is not None), w.kb))
                 if s._prev is not None:
                     wins.append(s._prev[None])
@@ -566,37 +767,89 @@ class StreamGroup:
                 s._feat = s._feat[drop:].clone()
                 s._feat0 += drop
 
-    def _decode(self, grp, flushed: bool):
+    def _decode(self, grp, flushed: bool, jobs=(), drain: bool = False):
         """Decode frames [emitted_frames, emit_end) of each stream of the group from its final latent with halo_dec
-        frames on each side; slices of equal length share one sab_decode.  Yields (stream, [2, samples])."""
+        frames on each side; slices of equal length share one sab_decode.  Yields (stream, [2, samples]).  Jobs' tiles
+        fill the call of steady slices, and their kept samples go to the job's output."""
         hop, halo = self.hop, self.halo_dec
-        jobs = []
+        items = []                              # (stream, latent rows, first kept sample, end sample, job output offset)
         for w in grp:
             s = w.key
             a, F = s.emitted_frames, s.final_frames
-            fl = flushed and w.last
+            fl = s._ends_at(w.kb)
             b = stream_emit_end(F, halo, fl)
             if b <= a:
-                jobs.append((s, None, 0, 0))
+                items.append((s, None, 0, 0, None))
                 continue
             d0, d1 = max(0, a - halo), F if fl else b + halo
-            jobs.append((s, s._lat[d0 - s._lat0:d1 - s._lat0], (a - d0) * hop, (b - d0) * hop))
+            items.append((s, s._lat[d0 - s._lat0:d1 - s._lat0], (a - d0) * hop, (b - d0) * hop, None))
             s.emitted_frames = b
             keep0 = max(0, b - halo)                               # the next decode reads from here on
             s._lat = s._lat[keep0 - s._lat0:].clone()
             s._lat0 = keep0
-        wavs = [None] * len(jobs)
         by_len = defaultdict(list)
-        for i, j in enumerate(jobs):
+        for i, j in enumerate(items):
             if j[1] is not None:
                 by_len[j[1].shape[0]].append(i)
+        steady = self._steady[1]
+        if drain:
+            by_len.setdefault(steady, [])                      # a drain tick has no live items: make the steady call
+        wavs = {}
         eng = self.model._ensure_engine()
         for T, idx in by_len.items():
-            slots = self._slots(len(idx), flushed, solve=False)
-            lat = torch.stack([jobs[idx[i]][1] for i in slots])
+            if T == steady and (jobs or drain):
+                slots, taken = self._call_slots(len(idx), flushed, False, jobs, SeparationJob._decode_offer, drain)
+                if slots is None:
+                    continue
+                for j, t in zip(jobs, taken):
+                    if not t:
+                        continue
+                    for start, k0, k1 in j._dec_tiles[j._dec_next:j._dec_next + t]:
+                        idx.append(len(items))
+                        items.append((j, j._lat[start - j._lat0:start - j._lat0 + T], (k0 - start) * hop,
+                                      (k1 - start) * hop, k0 * hop))
+                    j._dec_next += t
+                    # the next tile reads from its start on (the last, right-aligned, may start before this one's end)
+                    keep0 = j._dec_tiles[j._dec_next][0] if j._dec_next < len(j._dec_tiles) else j.final_frames
+                    j._lat = j._lat[keep0 - j._lat0:].clone()
+                    j._lat0 = keep0
+            else:
+                slots = self._slots(len(idx), flushed, solve=False)
+            lat = torch.stack([items[idx[i]][1] for i in slots])
             out = torch.empty(len(slots), 2, T * hop, device=self.device, dtype=torch.float32)
             eng.decode(lat, len(slots), T, out)
             for i, ji in enumerate(idx):
                 wavs[ji] = out[i]
-        for (s, _, a, b), wav in zip(jobs, wavs):
-            yield s, (torch.empty(2, 0, device=self.device) if wav is None else wav[:, a:b])
+        for i, (s, _, a, b, dst) in enumerate(items):
+            if dst is not None:
+                s._out[:, dst:dst + b - a].copy_(wavs[i][:, a:b])
+            else:
+                yield s, (torch.empty(2, 0, device=self.device) if i not in wavs else wavs[i][:, a:b])
+
+    def _finish_jobs(self, jobs):
+        """The jobs whose last tile has been decoded: their output at their own rate (one sab_resample call for all of
+        them), then their state is released and they leave the queue."""
+        sr = self.model.sample_rate
+        done = [j for j in jobs if not j.done and j._dec_next == len(j._dec_tiles)]
+        segs, outs = [], []
+        for j in done:
+            y = j._out
+            if j.sample_rate != sr:
+                n = y.shape[1]
+                y = torch.empty(2, resampled_length(n, sr, j.sample_rate), device=self.device, dtype=torch.float32)
+                segs += [dict(orig_rate=sr, new_rate=j.sample_rate, in_=j._out[r].data_ptr(), in_first=0, in_count=n,
+                              length=n, out=y[r].data_ptr(), out_first=0, out_count=y.shape[1]) for r in range(2)]
+            outs.append(y)
+        self.model._ensure_engine().resample(segs)
+        for j, y in zip(done, outs):
+            j._release()
+            j._result = StreamOutput(target=y[0], residual=y[1])
+            j.done = True
+            self._jobs.remove(j)
+
+
+def _drop_group(hold_plan_limits, key, jobs):
+    """Finalizer of a stream group collected without close(): cancel its jobs and give back its plan residency."""
+    for j in list(jobs):
+        j.cancel()
+    hold_plan_limits(key, None)

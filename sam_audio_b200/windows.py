@@ -157,6 +157,78 @@ def stream_flush_rows(budget_rows: int, W: int, resident: Sequence[int]) -> int:
     return min(int(budget_rows), max(resident) * int(W)) if resident else int(budget_rows)
 
 
+# ---- offline jobs in a stream group (StreamGroup.submit, DESIGN.md section 3) ----
+# A job is a stream whose whole input is known when it is submitted.  It runs only in the filler slots of a tick's
+# planned calls, so its codec slices must have the lengths of the plans those calls run: the steady slices of a live
+# stream (one window per tick).  Knowing its whole input, a job can cut every encode and decode into tiles of exactly
+# those lengths; a kept row sees the same operands as in an un-tiled run (DESIGN.md section 3, long clips), so the tiles
+# change no bit.
+
+
+def stream_steady_slices(W: int, halo_enc: int, halo_dec: int) -> Tuple[int, int]:
+    """Frames of a live stream's steady encode and decode slices, (H + 2 * halo_enc, H + 2 * halo_dec): the frames one
+    window adds, with the codec's halo on each side."""
+    H = stream_hop(W)
+    return H + 2 * int(halo_enc), H + 2 * int(halo_dec)
+
+
+def stream_job_min_frames(W: int, halo_enc: int, halo_dec: int) -> int:
+    """Latent frames a job needs so that both its encode and its decode can be cut into tiles of the steady lengths."""
+    return max(stream_steady_slices(W, halo_enc, halo_dec))
+
+
+def stream_tiles(n: int, L: int, halo: int) -> List[Tuple[int, int, int]]:
+    """Tiles of exactly L frames over frames [0, n): (start, keep0, keep1) per tile, the tile covering [start, start + L)
+    and keeping rows [keep0, keep1).  The first tile starts at 0 and the last ends at n (right-aligned); a tile keeps
+    the rows at least `halo` away from each of its cuts that is not an edge of [0, n), and the kept rows cover [0, n)
+    once, in order.  Needs n >= L > 2 * halo."""
+    n, L, halo = int(n), int(L), int(halo)
+    if L <= 2 * halo or n < L:
+        raise ValueError(f"tiles of {L} frames with a halo of {halo} over {n} frames: need n >= L > 2 * halo")
+    out: List[Tuple[int, int, int]] = []
+    a = 0
+    while a < n:
+        s = 0 if a == 0 else a - halo
+        if s + L >= n:                       # the tile reaches the end: right-align it, its kept rows start at a
+            out.append((n - L, a, n))
+            break
+        out.append((s, a, s + L - halo))
+        a = s + L - halo
+    return out
+
+
+def stream_job_admit(offers: Sequence[int], free: int) -> List[int]:
+    """Job items a planned call takes: offers[i] items are ready for the i-th job in submission order, and the call has
+    `free` filler slots.  First in, first out: a job gets slots only when every earlier job has none left ready; each
+    job's items are a prefix of its ready ones, so they keep their order."""
+    taken, free = [], max(0, int(free))
+    for n in offers:
+        t = min(max(0, int(n)), free)
+        taken.append(t)
+        free -= t
+    return taken
+
+
+def stream_job_slots(n_live: int, size: int, n_jobs: int) -> List[int]:
+    """Slots of a planned call of `size` slots with n_live live items and n_jobs job items: slot i < n_live + n_jobs
+    holds item i (live items first), every later slot repeats a live item as stream_bucket's filler does (a job item
+    when the call has none).  With n_jobs = 0 these are stream_bucket's slots."""
+    n_live, size, n_jobs = int(n_live), int(size), int(n_jobs)
+    n = n_live + n_jobs
+    if n_live < 0 or n_jobs < 0 or not 1 <= n <= size:
+        raise ValueError(f"{n_live} live and {n_jobs} job items in a call of {size} slots")
+    return [i if i < n else i % (n_live or n_jobs) for i in range(size)]
+
+
+def stream_drain_bucket(n: int, resident: Sequence[int]) -> int:
+    """Slots of a planned call of a tick that holds only jobs (StreamGroup.drain), with n job items ready: the smallest
+    resident bucket that holds them, else the largest (the rest wait for the next tick); bucket 1 when nothing is
+    resident, so draining plans no bucket that the group's live ticks have not."""
+    resident = [int(b) for b in resident] or [1]
+    fits = [b for b in resident if b >= int(n)]
+    return min(fits) if fits else max(resident)
+
+
 class TickWindows(NamedTuple):
     key: object    # the stream
     ka: int        # first window of the stream solved in this group
