@@ -351,6 +351,35 @@ int sab_resample(sab_engine* e, const sab_resample_seg* segs, int n_segs, void* 
 /* Host-only: the table sab_resample uses for a rate pair: *K taps, lo [n] (n = new / gcd) and, when w is not NULL,
  * w [n, K] fp32 (cap = floats w holds).  lo and w may be NULL to query K alone. */
 int sab_resample_taps(int orig_rate, int new_rate, int64_t cap, int* K, int* lo, float* w);
+/* Multichannel stems.  replaces: nothing — this goes beyond the reference, which is mono (its examples separate the
+ * channel mean); streams with keep_channels and SAMAudio.spread_channels() use it (DESIGN.md section 3).  At the
+ * codec's rate, with N = 2048, hop a = 512, the periodic Hann window w[n] = 0.5 - 0.5 cos(2 pi n / N) and frame j >= 0
+ * covering samples [j a - 3 a, j a + a): M_j[k] = (|T_j[k]|^2 + d) / (|T_j[k]|^2 + |R_j[k]|^2 + 2 d), d = 1e-10, from the
+ * rfft of the windowed mono target T and residual R; target_c[s] = (2/3) sum_j w[s - start_j] irfft(M_j X_c,j)[s -
+ * start_j] over the four frames covering s, ascending j, with X_c,j the rfft of the windowed channel c; residual_c[s] =
+ * x_c[s] - target_c[s] (one fp32 subtraction).  Samples outside a signal's known range are zero.  One call runs every
+ * segment in one launch; an output's bits depend only on its inputs, never on how the outputs are split into segments.
+ *  Each segment: 1 <= channels <= 8; target / residual hold samples [tr_first, tr_first + tr_count) of the mono stems
+ *  (tr_length = their length, < 0 = not known yet); mix [channels, mix_count] at mix_channel_stride holds samples
+ *  [mix_first, mix_first + mix_count) of the channels (mix_length likewise, at most tr_length when both are known);
+ *  outputs [out_first, out_first + out_count) go to out_target / out_residual [channels, out_count] at
+ *  out_channel_stride, and lie below tr_length when it is known.  Every input index an output reads must lie in its
+ *  window or past its signal's known end.  Every rule is checked on the host before any CUDA call; the descriptors go
+ *  to the device asynchronously on `stream` (calls of one engine must be ordered on one stream).  Not for graph
+ *  capture. */
+typedef struct sab_spread_seg {
+  int32_t struct_bytes;     /* = sizeof(sab_spread_seg), checked first */
+  int32_t channels;
+  const float* target;
+  const float* residual;
+  int64_t tr_first, tr_count, tr_length;
+  const float* mix;
+  int64_t mix_channel_stride, mix_first, mix_count, mix_length;
+  float* out_target;
+  float* out_residual;
+  int64_t out_channel_stride, out_first, out_count;
+} sab_spread_seg;
+int sab_spread_channels(sab_engine* e, const sab_spread_seg* segs, int n_segs, void* stream);
 
 /* host-only test seam: evaluation times of sab_solve's grid (method = SAB_ODE_*), in evaluation order */
 int sab_test_solver_grid(int method, int n_steps, int cap, int* n_evals, float* times);

@@ -96,11 +96,29 @@ class SabResampleSeg(ctypes.Structure):
             setattr(self, k, v)
 
 
+class SabSpreadSeg(ctypes.Structure):
+    """Mirror of sab_spread_seg (include/samaudio_b200.h); pointers are device addresses as ints."""
+    _i32, _i64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
+    _fields_ = [("struct_bytes", _i32), ("channels", _i32),
+                ("target", _vp), ("residual", _vp), ("tr_first", _i64), ("tr_count", _i64), ("tr_length", _i64),
+                ("mix", _vp), ("mix_channel_stride", _i64), ("mix_first", _i64), ("mix_count", _i64),
+                ("mix_length", _i64),
+                ("out_target", _vp), ("out_residual", _vp), ("out_channel_stride", _i64), ("out_first", _i64),
+                ("out_count", _i64)]
+
+    def __init__(self, **kw):
+        super().__init__()
+        self.struct_bytes = ctypes.sizeof(SabSpreadSeg)
+        self.channels, self.tr_length, self.mix_length = 1, -1, -1
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
 EXPORTS = [
     "sab_last_error", "sab_version", "sab_create", "sab_destroy", "sab_load_weight", "sab_finalize_weights",
     "sab_encode", "sab_prepare", "sab_dit_forward", "sab_solve", "sab_decode", "sab_launch_count",
     "sab_workspace_bytes", "sab_set_plan_limits", "sab_plan_stats", "sab_profile", "sab_profile_report", "sab_test_gemm", "sab_test_gemm_ex", "sab_test_xattn_fold", "sab_test_attention", "sab_test_attention_tc2", "sab_test_attention_stream", "sab_codec_tiling", "sab_preprocess_frames", "sab_blend_windows", "sab_test_aa_taps", "sab_test_solver_grid",
-    "sab_resample", "sab_resample_taps",
+    "sab_resample", "sab_resample_taps", "sab_spread_channels",
     "sab_test_rmsnorm_mod", "sab_test_group_norm_silu", "sab_test_time_features", "sab_test_cond_finish",
     "sab_test_rope_table", "sab_test_codec_end", "sab_test_attention_cross", "sab_test_t5_norm", "sab_test_t5_attention",
     "sab_t5_create", "sab_t5_destroy", "sab_t5_load_weight", "sab_t5_finalize", "sab_t5_forward", "sab_t5_launch_count",
@@ -153,6 +171,7 @@ def lib() -> ctypes.CDLL:
         L.sab_test_solver_grid.argtypes = [i32, i32, i32, vp, vp]
         L.sab_resample.argtypes = [vp, ctypes.POINTER(SabResampleSeg), i32, vp]
         L.sab_resample_taps.argtypes = [i32, i32, i64, ctypes.POINTER(i32), vp, vp]
+        L.sab_spread_channels.argtypes = [vp, ctypes.POINTER(SabSpreadSeg), i32, vp]
         f32 = ctypes.c_float
         L.sab_test_rmsnorm_mod.argtypes = [i32, i32, vp, vp, vp, vp, i64, i32, f32, i32, vp, vp]
         L.sab_test_group_norm_silu.argtypes = [i32, i64, i32, vp, vp, vp, f32, vp, vp]
@@ -264,6 +283,14 @@ def resample_segments(segs) -> ctypes.Array:
     return arr
 
 
+def spread_segments(segs) -> ctypes.Array:
+    """A list of SabSpreadSeg (or of dicts of its fields) as the C array sab_spread_channels takes."""
+    arr = (SabSpreadSeg * max(1, len(segs)))()
+    for i, s in enumerate(segs):
+        arr[i] = s if isinstance(s, SabSpreadSeg) else SabSpreadSeg(**s)
+    return arr
+
+
 class Engine:
     """Owns one sab_engine handle."""
 
@@ -345,6 +372,11 @@ class Engine:
         """One sab_resample launch over `segs` (SabResampleSeg or dicts of its fields) on the current stream."""
         if segs:
             check(lib().sab_resample(self._h, resample_segments(segs), len(segs), stream_ptr()))
+
+    def spread_channels(self, segs) -> None:
+        """One sab_spread_channels launch over `segs` (SabSpreadSeg or dicts of its fields) on the current stream."""
+        if segs:
+            check(lib().sab_spread_channels(self._h, spread_segments(segs), len(segs), stream_ptr()))
 
     DEFAULT_PLAN_LIMITS = (1, 3)    # include/samaudio_b200.h sab_set_plan_limits
 

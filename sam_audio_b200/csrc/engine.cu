@@ -22,6 +22,7 @@
 #include "xattn_fold.cuh"
 #include "blend_windows.cuh"
 #include "resample.cuh"
+#include "spread_channels.cuh"
 
 using namespace sab;
 typedef __nv_bfloat16 bf16;
@@ -431,6 +432,13 @@ struct sab_engine {
   DevicePool rs_desc_pool;
   ResampleSeg* rs_desc = nullptr;
   int64_t rs_desc_cap = 0;
+
+  // sab_spread_channels: the twiddle and window table (built on first use, kept until sab_destroy) and the device copy
+  // of a call's segment list
+  DevicePool sp_table_pool, sp_desc_pool;
+  float2* sp_table = nullptr;
+  SpreadSeg* sp_desc = nullptr;
+  int64_t sp_desc_cap = 0;
 
   ~sab_engine();
 };
@@ -2165,7 +2173,7 @@ int64_t sab_workspace_bytes(sab_engine* e) {
   for (auto& kv : e->enc_plans) b += kv.second->pool.bytes;
   for (auto& kv : e->dec_plans) b += kv.second->pool.bytes;
   for (auto& kv : e->rs_tables) b += kv.second->pool.bytes;
-  return b + e->rs_desc_pool.bytes;
+  return b + e->rs_desc_pool.bytes + e->sp_table_pool.bytes + e->sp_desc_pool.bytes;
 }
 
 int sab_set_plan_limits(sab_engine* e, int dit_plans, int codec_plans_per_direction) {
@@ -2825,6 +2833,113 @@ int sab_resample(sab_engine* e, const sab_resample_seg* segs, int n_segs, void* 
   ensure_dynamic_smem(reinterpret_cast<const void*>(resample_kernel), RS_MAX_SMEM);
   mark(e, st, "resample", 0, bytes);
   resample_kernel<<<(unsigned)ctas, RS_THREADS, (size_t)smem, st>>>(e->rs_desc, (int)dev.size(), (int)tab_floats);
+  SAB_CUDA(cudaGetLastError());
+  SAB_API_END
+}
+
+// ---- multichannel stems (spread_channels.cuh) ----
+// The twiddles exp(-2 pi i m / N), m < N / 2, then the periodic Hann window, evaluated in float64 and rounded once.
+static const float2* spread_table_dev(sab_engine* e) {
+  if (!e->sp_table) {
+    std::vector<float2> h(SP_N / 2 + SP_N / 2);          // N / 2 twiddles, then N window floats as N / 2 float2
+    float* win = reinterpret_cast<float*>(h.data() + SP_N / 2);
+    const double pi = 3.14159265358979323846;
+    for (int m = 0; m < SP_N / 2; ++m)
+      h[m] = make_float2((float)cos(2.0 * pi * m / SP_N), (float)-sin(2.0 * pi * m / SP_N));
+    for (int n = 0; n < SP_N; ++n) win[n] = (float)(0.5 - 0.5 * cos(2.0 * pi * n / SP_N));
+    float2* d = e->sp_table_pool.alloc<float2>((int64_t)h.size());
+    SAB_CUDA(cudaMemcpy(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice));
+    e->sp_table = d;
+  }
+  return e->sp_table;
+}
+
+// Does the window [first, first + count) of a signal of `length` samples (< 0: unknown) hold every index of [a, b)
+// that is >= 0 and below the known length?
+static bool spread_window_holds(int64_t first, int64_t count, int64_t length, int64_t a, int64_t b) {
+  a = a < 0 ? 0 : a;
+  if (length >= 0) b = b < length ? b : length;
+  return a >= b || (a >= first && b <= first + count);
+}
+
+int sab_spread_channels(sab_engine* e, const sab_spread_seg* segs, int n_segs, void* stream) {
+  SAB_API_BEGIN
+  SAB_CHECK(n_segs >= 0 && (segs || n_segs == 0), "bad segment list (n_segs=%d)", n_segs);
+  for (int i = 0; i < n_segs; ++i) {
+    const sab_spread_seg& g = segs[i];
+    SAB_CHECK(g.struct_bytes == (int32_t)sizeof(sab_spread_seg),
+              "sab_spread_seg.struct_bytes=%d but the library's descriptor has %d bytes (header and binding differ)",
+              g.struct_bytes, (int)sizeof(sab_spread_seg));
+    SAB_CHECK(g.channels >= 1 && g.channels <= 8, "segment %d: channels=%d outside 1..8", i, g.channels);
+    SAB_CHECK(g.tr_count >= 0 && g.mix_count >= 0 && g.out_count >= 0 && g.out_first >= 0 && g.tr_length >= -1 &&
+                  g.mix_length >= -1,
+              "segment %d: negative count (tr_count=%lld, mix_count=%lld, out_first=%lld, out_count=%lld, "
+              "tr_length=%lld, mix_length=%lld)", i, (long long)g.tr_count, (long long)g.mix_count,
+              (long long)g.out_first, (long long)g.out_count, (long long)g.tr_length, (long long)g.mix_length);
+    SAB_CHECK(g.channels == 1 || g.mix_channel_stride >= g.mix_count, "segment %d: mix channel stride %lld < mix_count %lld",
+              i, (long long)g.mix_channel_stride, (long long)g.mix_count);
+    SAB_CHECK(g.channels == 1 || g.out_channel_stride >= g.out_count,
+              "segment %d: output channel stride %lld < out_count %lld", i, (long long)g.out_channel_stride,
+              (long long)g.out_count);
+    SAB_CHECK(g.tr_length < 0 || g.mix_length < 0 || g.mix_length <= g.tr_length,
+              "segment %d: a mixture of %lld samples is longer than its %lld-sample stems", i, (long long)g.mix_length,
+              (long long)g.tr_length);
+    if (g.out_count == 0) continue;
+    SAB_CHECK(g.out_target && g.out_residual, "segment %d: null output", i);
+    SAB_CHECK(g.tr_length < 0 || g.out_first + g.out_count <= g.tr_length,
+              "segment %d: outputs [%lld, %lld) past the end of %lld-sample stems", i, (long long)g.out_first,
+              (long long)(g.out_first + g.out_count), (long long)g.tr_length);
+    // outputs [s0, s1) read the frames floor(s0 / a) .. floor((s1 - 1) / a) + 3
+    const int64_t s0 = g.out_first, s1 = g.out_first + g.out_count;
+    const int64_t a = (s0 / SP_HOP - 3) * SP_HOP, b = ((s1 - 1) / SP_HOP + 4) * SP_HOP;
+    const int64_t bt = g.tr_length >= 0 && g.tr_length < b ? g.tr_length : b;
+    const int64_t bx = g.mix_length >= 0 && g.mix_length < b ? g.mix_length : b;
+    SAB_CHECK(spread_window_holds(g.tr_first, g.tr_count, g.tr_length, a, b),
+              "segment %d: outputs [%lld, %lld) read stem samples [%lld, %lld), the buffers hold [%lld, %lld) (length "
+              "%lld)", i, (long long)s0, (long long)s1, (long long)(a < 0 ? 0 : a), (long long)bt, (long long)g.tr_first,
+              (long long)(g.tr_first + g.tr_count), (long long)g.tr_length);
+    SAB_CHECK(spread_window_holds(g.mix_first, g.mix_count, g.mix_length, a, b),
+              "segment %d: outputs [%lld, %lld) read mixture samples [%lld, %lld), the buffer holds [%lld, %lld) "
+              "(length %lld)", i, (long long)s0, (long long)s1, (long long)(a < 0 ? 0 : a), (long long)bx,
+              (long long)g.mix_first, (long long)(g.mix_first + g.mix_count), (long long)g.mix_length);
+    SAB_CHECK((g.target && g.residual) || spread_window_holds(0, 0, g.tr_length, a, b), "segment %d: null stems", i);
+    SAB_CHECK(g.mix || spread_window_holds(0, 0, g.mix_length, a, b), "segment %d: null mixture", i);
+    SAB_CHECK(g.out_count <= (int64_t)SP_SPAN * (INT32_MAX / 2), "segment %d: %lld outputs is too many for one call", i,
+              (long long)g.out_count);
+  }
+  SAB_CHECK(e != nullptr, "null engine");
+  DeviceGuard _dg(e->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<SpreadSeg> dev;
+  int64_t ctas = 0;
+  int c_max = 1;
+  double bytes = 0;
+  for (int i = 0; i < n_segs; ++i) {
+    const sab_spread_seg& g = segs[i];
+    if (g.out_count == 0) continue;
+    SpreadSeg s{g.target, g.residual, g.tr_first, g.tr_count, g.tr_length, g.mix, g.mix_channel_stride, g.mix_first,
+                g.mix_count, g.mix_length, g.out_target, g.out_residual, g.out_channel_stride, g.out_first, g.out_count,
+                g.channels, (int)ctas};
+    dev.push_back(s);
+    const int64_t h0 = g.out_first / SP_HOP, h1 = (g.out_first + g.out_count - 1) / SP_HOP;
+    ctas += (h1 - h0) / SP_HOPS + 1;
+    c_max = std::max(c_max, (int)g.channels);
+    bytes += 4.0 * (double)g.out_count * (2.0 + 3.0 * g.channels);
+  }
+  SAB_CHECK(ctas <= INT32_MAX, "%lld CTAs is too many for one call", (long long)ctas);
+  if (dev.empty()) return 0;
+  const float2* table = spread_table_dev(e);
+  if ((int64_t)dev.size() > e->sp_desc_cap) {
+    SAB_CUDA(cudaStreamSynchronize(st));           // the old list may still be read by an earlier launch
+    e->sp_desc_pool.release();
+    e->sp_desc_cap = std::max<int64_t>(64, (int64_t)dev.size());
+    e->sp_desc = e->sp_desc_pool.alloc<SpreadSeg>(e->sp_desc_cap);
+  }
+  SAB_CUDA(cudaMemcpyAsync(e->sp_desc, dev.data(), dev.size() * sizeof(SpreadSeg), cudaMemcpyHostToDevice, st));
+  ensure_dynamic_smem(reinterpret_cast<const void*>(spread_channels_kernel), SP_MAX_SMEM);
+  const int64_t smem = SP_SMEM_FIXED + (int64_t)c_max * SP_SPAN * (int64_t)sizeof(float);
+  mark(e, st, "spread_channels", 0, bytes);
+  spread_channels_kernel<<<(unsigned)ctas, SP_THREADS, (size_t)smem, st>>>(e->sp_desc, (int)dev.size(), table);
   SAB_CUDA(cudaGetLastError());
   SAB_API_END
 }

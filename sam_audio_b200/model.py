@@ -401,6 +401,35 @@ class SAMAudio(torch.nn.Module):
             self._ensure_engine().resample(segs)
         return out if wav.dim() == 2 else out[0]
 
+    @torch.inference_mode()
+    def spread_channels(self, target: torch.Tensor, residual: torch.Tensor, mixture: torch.Tensor):
+        """Stereo and surround stems from one mono separation (sab_spread_channels, DESIGN.md section 3): the mono
+        target and residual define a time-frequency Wiener mask (STFT of 2048 samples, hop 512, periodic Hann), and the
+        mask is applied to every channel of the mixture, so the stems keep its spatial image:
+
+            x48 = model.resample(wav, 44100, model.sample_rate)            # [C, S] channels at the codec's rate
+            out = model.separate(processor(descriptions=["piano"], audios=[x48.mean(0, keepdim=True)]).to("cuda"))
+            tgt, res = model.spread_channels(out.target[0], out.residual[0], x48)   # [C, S'] each
+
+        target, residual: fp32 [S'] at the model's rate on its CUDA device; mixture: fp32 [C, S], 1 <= C <= 8,
+        1 <= S <= S' (zero past S).  Returns (target [C, S'], residual [C, S']) with residual = mixture - target in
+        each channel, one fp32 subtraction, all in one launch."""
+        from .channels import check_spread_shapes
+        C, S, S2 = check_spread_shapes(target, residual, mixture)
+        for t in (target, residual, mixture):
+            if t.dtype != torch.float32 or t.device != self._device or self._device.type != "cuda":
+                raise ValueError(f"spread_channels() takes fp32 samples on the model's CUDA device ({self._device}), "
+                                 f"got {t.dtype} on {t.device}")
+        t, r, x = target.contiguous(), residual.contiguous(), mixture.contiguous()
+        out = torch.empty(2, C, S2, device=t.device, dtype=torch.float32)
+        seg = dict(channels=C, target=t.data_ptr(), residual=r.data_ptr(), tr_first=0, tr_count=S2, tr_length=S2,
+                   mix=x.data_ptr(), mix_channel_stride=S, mix_first=0, mix_count=S, mix_length=S,
+                   out_target=out[0].data_ptr(), out_residual=out[1].data_ptr(), out_channel_stride=S2, out_first=0,
+                   out_count=S2)
+        with torch.cuda.device(t.device):
+            self._ensure_engine().spread_channels([seg])
+        return out[0], out[1]
+
     def _stream_args(self, window_seconds: float, ode_opt: Dict[str, Any], reranking_candidates: int, anchors,
                      masked_video):
         """(W, n_steps, method) of a stream, after the checks stream() and stream_group() share."""
@@ -421,7 +450,7 @@ class SAMAudio(torch.nn.Module):
 
     def stream(self, description: str, window_seconds: float = 10.0, seed: int = 0,
                ode_opt: Dict[str, Any] = DFLT_ODE_OPT, reranking_candidates: int = 1, anchors=None,
-               masked_video=None, sample_rate: Optional[int] = None):
+               masked_video=None, sample_rate: Optional[int] = None, keep_channels: bool = False):
         """Separation of audio that arrives in chunks (sam_audio_b200.stream, DESIGN.md section 3):
 
             s = model.stream(description="man speaking", sample_rate=16000)
@@ -434,6 +463,14 @@ class SAMAudio(torch.nn.Module):
         resample(out, model rate, sample_rate) of the model-rate stream pushed resample(channel mean, sample_rate, model
         rate), whatever the chunking.
 
+        keep_channels=True: the outputs are [C, S], the stems of every pushed channel (C from the first push).  The mono
+        separation above runs unchanged, and its model-rate target and residual define a Wiener mask that is applied to
+        each channel at the model's rate (spread_channels), so the stems keep the input's spatial image and each
+        channel's target and residual sum to that channel.  The output equals, bit for bit, resample(spread_channels(T,
+        R, x), model rate, sample_rate), with T, R the model-rate stream's output and x the channels at the model's rate
+        (resample(x, sample_rate, model rate) row by row), whatever the chunking.  It adds at most 2048 samples at the
+        model's rate (42.7 ms) of latency.
+
         The stream is solved as windows of W = round(window_seconds * 25) latent frames, 8 <= W <= max_positions; the
         default 10 s keeps the DiT on its short-sequence attention (T <= 256).  Text prompts with one candidate only.
         The stream is the one stream of a group of its own (stream_group) that keeps the engine's default plan
@@ -445,8 +482,11 @@ class SAMAudio(torch.nn.Module):
         if sample_rate is not None:
             from .resample import check_rate
             check_rate(sample_rate)
+        from .stream import check_keep_channels
+        check_keep_channels(keep_channels)
         return StreamGroup(self, W, n_steps, method, resident_plans=False).open(description, seed=int(seed),
-                                                                                 sample_rate=sample_rate)
+                                                                                 sample_rate=sample_rate,
+                                                                                 keep_channels=keep_channels)
 
     def stream_group(self, window_seconds: float = 10.0, ode_opt: Dict[str, Any] = DFLT_ODE_OPT,
                      reranking_candidates: int = 1, anchors=None, masked_video=None):
@@ -455,6 +495,7 @@ class SAMAudio(torch.nn.Module):
             group = model.stream_group(window_seconds=10.0)
             a = group.open("man speaking", seed=0)      # a stream, with push / flush as from stream()
             c = group.open("rain", sample_rate=16000)    # ... at its own rate and channel count
+            d = group.open("piano", keep_channels=True)  # ... with [C, S] stems of every channel (see stream())
             b = group.open("dog barking", seed=7)
             outs = group.push({a: chunk_a, b: chunk_b})  # one tick -> {stream: StreamOutput}
             tails = group.flush([a, b])                  # ends and closes them (a.flush() alone works too)
@@ -473,6 +514,7 @@ class SAMAudio(torch.nn.Module):
         Offline jobs take the ticks' filler slots (the spare slots of each bucket, otherwise repeated live items):
 
             job = group.submit(wav, "dog barking", seed=3, sample_rate=16000)   # a whole recording, [S] or [C, S]
+                                                                                # (keep_channels as for open())
             group.drain([job])                   # ticks of jobs only, at buckets the group uses; close() drains too
             out = job.result()                   # == model.stream(...) with wav pushed once and flushed, bit for bit
 

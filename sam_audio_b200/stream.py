@@ -37,6 +37,11 @@ know their lengths and apply the zero fill at the end.  In a tick every stream's
 the encode and every stream's output one call after the decode.  Each resampler holds at most K samples plus one push
 (K = its table's taps).  A mono stream at the codec's rate has neither.  PyTorch only allocates, slices and
 concatenates here; the arithmetic runs in libsamaudio_b200.so.
+
+A stream with keep_channels also brings every channel to the codec's rate (a per-channel resampler, in the same ingest
+launch) and runs a multichannel stage between the decode and the output resampler (_Spread, sab_spread_channels,
+sam_audio_b200.channels): the mono target and residual define a Wiener mask applied to each channel, and a sample is
+emitted once its last frame's inputs are known.  In a tick every such stream's stage is one sab_spread_channels call.
 """
 from __future__ import annotations
 
@@ -48,6 +53,7 @@ from typing import Dict, Iterable, List, Mapping
 import torch
 
 from . import _capi
+from .channels import keep_from, spread_ready
 from .resample import check_rate, first_tap, outputs_ready, resampled_length, taps
 from .windows import (TickWindows, stream_bucket, stream_drain_bucket, stream_emit_end, stream_final_frames,
                       stream_flush_rows, stream_frames_available, stream_group_capacity, stream_hop, stream_job_admit,
@@ -59,8 +65,9 @@ _NULL_ANCHOR_IDS = (0, 3)   # the processor's ids of a clip without anchors: <nu
 
 @dataclass
 class StreamOutput:
-    target: torch.Tensor     # [S] samples of the separated source that became final with this call
-    residual: torch.Tensor   # [S] the rest of the mixture over the same samples
+    target: torch.Tensor     # [S] samples of the separated source that became final with this call ([C, S] for a
+                             # stream or job with keep_channels)
+    residual: torch.Tensor   # [S] the rest of the mixture over the same samples ([C, S] likewise)
 
 
 def _block_seed(seed: int, block: int) -> int:
@@ -170,19 +177,93 @@ class _Resampler:
         self.first = keep0
 
 
+class _Rows:
+    """Samples [first, received) of `rows` signals on the device, in buf[:, :received - first]; spare has the same size
+    and takes the kept samples on a trim, so a stream in steady state allocates nothing."""
+
+    def __init__(self, rows: int, device):
+        self.rows, self.device = rows, device
+        self.buf = self._spare = None
+        self.first = self.received = 0
+
+    def append(self, x: torch.Tensor):
+        held, S = self.received - self.first, x.shape[1]
+        if self.buf is None or held + S > self.buf.shape[1]:
+            buf = torch.empty(self.rows, 2 * (held + S), device=self.device, dtype=torch.float32)
+            if held:
+                buf[:, :held].copy_(self.buf[:, :held])
+            self.buf, self._spare = buf, torch.empty_like(buf)
+        self.buf[:, held:held + S].copy_(x)
+        self.received += S
+
+    def trim(self, keep0: int):
+        keep0 = min(self.received, keep0)
+        if keep0 <= self.first:
+            return
+        a, b = keep0 - self.first, self.received - self.first
+        self._spare[:, :b - a].copy_(self.buf[:, a:b])
+        self.buf, self._spare = self._spare, self.buf
+        self.first = keep0
+
+    def ptr(self, row: int = 0) -> int:
+        return 0 if self.buf is None else self.buf[row].data_ptr()
+
+
+class _Spread:
+    """The multichannel stage of a keep-channels stream (sab_spread_channels, sam_audio_b200.channels): the codec-rate
+    mono target and residual as they become final (tr, 2 rows), the codec-rate channels as they arrive (x, C rows), and
+    the outputs [0, produced) made so far.  The lengths are known at flush().  Holds, per row, the samples the next
+    output's frames read: the mono stream's delay plus N samples."""
+
+    def __init__(self, C: int, device):
+        self.C, self.device = C, device
+        self.tr, self.x = _Rows(2, device), _Rows(C, device)
+        self.tr_length = self.x_length = None
+        self.produced = 0
+
+    def take(self):
+        """(segment, out): the sab_spread_channels segment of the outputs that became computable (None if there are
+        none) and their output tensor [2, C, count] (target, residual)."""
+        q0 = self.produced
+        q1 = max(q0, spread_ready(self.tr.received, self.x.received, self.tr_length, self.x_length))
+        out = torch.empty(2, self.C, q1 - q0, device=self.device, dtype=torch.float32)
+        seg = None
+        if q1 > q0:
+            tr, x = self.tr, self.x
+            seg = dict(channels=self.C, target=tr.ptr(0), residual=tr.ptr(1), tr_first=tr.first,
+                       tr_count=tr.received - tr.first, tr_length=-1 if self.tr_length is None else self.tr_length,
+                       mix=x.ptr(), mix_channel_stride=0 if x.buf is None else x.buf.shape[1], mix_first=x.first,
+                       mix_count=x.received - x.first, mix_length=-1 if self.x_length is None else self.x_length,
+                       out_target=out[0].data_ptr(), out_residual=out[1].data_ptr(), out_channel_stride=q1 - q0,
+                       out_first=q0, out_count=q1 - q0)
+        self.produced = q1
+        return seg, out
+
+    def trim(self):
+        """Drop the inputs no later output reads (after the launch that read them is enqueued)."""
+        k = keep_from(self.produced)
+        self.tr.trim(k)
+        self.x.trim(k)
+
+
 class SeparationStream:
     """Returned by ``SAMAudio.stream()`` and ``StreamGroup.open()``; see there.  ``push`` returns the samples that became
     final, ``flush`` the rest, and the concatenation of everything returned is ceil(n / hop) * hop samples for n samples
     pushed.  ``push`` and ``flush`` are ticks of the stream's group with this stream alone."""
 
-    def __init__(self, group: "StreamGroup", description: str, seed: int, sample_rate: int):
+    def __init__(self, group: "StreamGroup", description: str, seed: int, sample_rate: int,
+                 keep_channels: bool = False):
         self.group = group
         self.model = group.model
         self.sample_rate = sample_rate                         # of push() and of the outputs
+        self.keep_channels = keep_channels                     # outputs [C, S]: the stems of every pushed channel
         self.channels = None                                   # of push(), fixed by the first
         self._ingest = None                                    # resampler to the codec's rate (set by the first push)
+        self._split = None                                     # keep_channels: per-channel resampler to the codec's rate
+        self._spread = None                                    # keep_channels: the multichannel stage (_Spread)
         sr = self.model.sample_rate
-        self._emit = None if sample_rate == sr else _Resampler(sr, sample_rate, 2, False, group.device)
+        # the output resampler: mono target and residual, or (keep_channels) 2 C rows made at the first push
+        self._emit = None if sample_rate == sr or keep_channels else _Resampler(sr, sample_rate, 2, False, group.device)
         self.W, self.O, self.H, self.hop, self.C = group.W, group.O, group.H, group.hop, group.C
         self.seed = seed
         self.device = group.device
@@ -260,7 +341,7 @@ class SeparationStream:
 
     def _release(self):
         self._buf = self._spare = self._feat = self._lat = self._prev = None
-        self._ingest = self._emit = None
+        self._ingest = self._emit = self._split = self._spread = None
 
     def _set_channels(self, C: int):
         if self.channels is None:
@@ -268,6 +349,11 @@ class SeparationStream:
             sr = self.model.sample_rate
             if self.sample_rate != sr or C > 1:
                 self._ingest = _Resampler(self.sample_rate, sr, C, True, self.device)
+            if self.keep_channels:
+                self._spread = _Spread(C, self.device)
+                if self.sample_rate != sr:
+                    self._split = _Resampler(self.sample_rate, sr, C, False, self.device)
+                    self._emit = _Resampler(sr, self.sample_rate, 2 * C, False, self.device)
 
     def _output(self, pieces: List[torch.Tensor]) -> StreamOutput:
         if not pieces:
@@ -290,10 +376,12 @@ class SeparationJob:
     _text_at = SeparationStream._text_at
     _ends_at = SeparationStream._ends_at
 
-    def __init__(self, group: "StreamGroup", description: str, seed: int, sample_rate: int, wav: torch.Tensor):
+    def __init__(self, group: "StreamGroup", description: str, seed: int, sample_rate: int, wav: torch.Tensor,
+                 keep_channels: bool = False):
         self._group = weakref.ref(group)      # the group's finalizer cancels its jobs, so a job must not keep it alive
         self.model = group.model
         self.sample_rate = sample_rate
+        self.keep_channels = keep_channels
         self.W, self.O, self.H, self.hop, self.C = group.W, group.O, group.H, group.hop, group.C
         self.seed = seed
         self.device = group.device
@@ -303,18 +391,27 @@ class SeparationJob:
         self._text_mask = tm.to(self.device).contiguous()
         self.n_tokens = self._text.shape[1]
         sr = self.model.sample_rate
+        self._x48 = None                                       # keep_channels: the channels at the codec's rate [C, n]
         with torch.cuda.device(self.device):
             if sample_rate != sr or wav.shape[0] > 1:        # the stream's ingest, with the whole length known
                 x = wav.to(device=self.device, dtype=torch.float32).contiguous()
                 S = x.shape[1]
                 x48 = torch.empty(1, resampled_length(S, sample_rate, sr), device=self.device, dtype=torch.float32)
-                self.model._ensure_engine().resample([dict(
-                    orig_rate=sample_rate, new_rate=sr, channels=x.shape[0], in_=x.data_ptr(), in_channel_stride=S,
-                    in_first=0, in_count=S, length=S, out=x48.data_ptr(), out_first=0, out_count=x48.shape[1])])
+                seg = dict(orig_rate=sample_rate, new_rate=sr, in_first=0, in_count=S, length=S, out_first=0,
+                           out_count=x48.shape[1])
+                segs = [dict(seg, channels=x.shape[0], in_=x.data_ptr(), in_channel_stride=S, out=x48.data_ptr())]
+                if keep_channels and sample_rate != sr:        # ... and the per-channel one, in the same launch
+                    self._x48 = torch.empty(x.shape[0], x48.shape[1], device=self.device, dtype=torch.float32)
+                    segs += [dict(seg, in_=x[c].data_ptr(), out=self._x48[c].data_ptr()) for c in range(x.shape[0])]
+                elif keep_channels:
+                    self._x48 = wav.to(device=self.device, dtype=torch.float32, copy=True).contiguous()
+                self.model._ensure_engine().resample(segs)
             else:
                 # a copy, as push() makes one: the tiles read the recording over later ticks, and the caller may reuse
                 # its tensor as soon as submit() returns
                 x48 = wav.to(device=self.device, dtype=torch.float32, copy=True).contiguous()
+                if keep_channels:
+                    self._x48 = x48
             self._wav = self.model._pad(x48)[0]               # reflect-padded to n_final frames, as flush() pads
         self.n_samples = x48.shape[1]
         self._init_schedule(-(-self.n_samples // self.hop), group.halo_enc, group.halo_dec)
@@ -377,6 +474,7 @@ class SeparationJob:
 
     def _release(self):
         self._wav = self._feat = self._lat = self._prev = self._out = self._text = self._text_mask = None
+        self._x48 = None
 
 
 class StreamGroup:
@@ -414,30 +512,35 @@ class StreamGroup:
             self._finalizer.atexit = False
 
     # ------------------------------------------------------------------ public
-    def open(self, description: str, seed: int = 0, sample_rate=None) -> SeparationStream:
+    def open(self, description: str, seed: int = 0, sample_rate=None, keep_channels: bool = False) -> SeparationStream:
         """A new stream of the group with its own prompt and noise seed.  sample_rate: of its pushes and outputs (an
-        integer in [8000, 192000] Hz; None: the model's rate)."""
+        integer in [8000, 192000] Hz; None: the model's rate).  keep_channels: the outputs are [C, S], the stems of
+        every pushed channel (SAMAudio.stream)."""
         if self.closed:
             raise RuntimeError("the stream group is closed")
         if not isinstance(description, str):
             raise TypeError("a stream separates one source: description must be one string")
+        keep_channels = check_keep_channels(keep_channels)
         sr = self.model.sample_rate if sample_rate is None else check_rate(sample_rate)
-        s = SeparationStream(self, description, int(seed), sr)
+        s = SeparationStream(self, description, int(seed), sr, keep_channels)
         self.L = max(self.L, s.n_tokens)
         self.streams.append(s)
         return s
 
     @torch.inference_mode()
-    def submit(self, wav: torch.Tensor, description: str, seed: int = 0, sample_rate=None) -> SeparationJob:
+    def submit(self, wav: torch.Tensor, description: str, seed: int = 0, sample_rate=None,
+               keep_channels: bool = False) -> SeparationJob:
         """Queue a whole recording ([S], [1, S] or [C, S] with C <= 8, at sample_rate) to be separated in the idle slots
-        of the group's ticks; see SeparationJob.  sample_rate and the prompt are as for open() (the prompt counts
-        toward the group's text length: a prompt longer than every earlier one makes the next tick re-plan its buckets
-        at the new length, as open() does).  The recording is copied, so the caller may reuse its tensor at once.  It
-        must be long enough to be cut into codec tiles of the steady slice lengths (stream_job_min_frames)."""
+        of the group's ticks; see SeparationJob.  sample_rate, keep_channels and the prompt are as for open() (the
+        prompt counts toward the group's text length: a prompt longer than every earlier one makes the next tick
+        re-plan its buckets at the new length, as open() does).  The recording is copied, so the caller may reuse its
+        tensor at once.  It must be long enough to be cut into codec tiles of the steady slice lengths
+        (stream_job_min_frames)."""
         if self.closed:
             raise RuntimeError("the stream group is closed")
         if not isinstance(description, str):
             raise TypeError("a job separates one source: description must be one string")
+        keep_channels = check_keep_channels(keep_channels)
         sr = self.model.sample_rate if sample_rate is None else check_rate(sample_rate)
         x = _samples(wav, what="submit()")
         n48 = x.shape[1] if sr == self.model.sample_rate else resampled_length(x.shape[1], sr, self.model.sample_rate)
@@ -446,7 +549,7 @@ class StreamGroup:
             raise ValueError(f"a job of {x.shape[1] / sr:.3f} s is too short: a stream group's jobs need at least "
                              f"{need * self.hop / self.model.sample_rate:.3f} s ({need} latent frames) at this window "
                              "length; separate() or stream() take shorter recordings")
-        job = SeparationJob(self, description, int(seed), sr, x)
+        job = SeparationJob(self, description, int(seed), sr, x, keep_channels)
         self.L = max(self.L, job.n_tokens)
         self._jobs.append(job)
         return job
@@ -475,15 +578,18 @@ class StreamGroup:
         with torch.cuda.device(self.device):
             for s, x in zip(streams, xs):
                 s._set_channels(x.shape[0])
-            ingested = self._resample_in(streams, xs, flushed=False)
+            ingested, split = self._resample_in(streams, xs, flushed=False)
             due = []
             for s, x in zip(streams, xs):
                 s._append(ingested.get(s, x[0]))
+                if s._spread is not None:
+                    s._spread.x.append(split.get(s, x))
                 avail = stream_frames_available(s.n_samples, self.hop, self.halo_enc)
                 due.append((s, s.windows_solved, stream_windows_ready(avail, self.W)))
             out = self._tick(due, flushed=False)
             for s in streams:
                 s._trim_samples()
+            out = self._spread_out(out, flushed=False)
             out = self._resample_out(out, flushed=False)
         return out
 
@@ -495,9 +601,13 @@ class StreamGroup:
         try:
             with torch.cuda.device(self.device):
                 # the ingest's zero fill at the end: the codec-rate stream gets the rest of its samples first
-                for s, x in self._resample_in(streams, [None] * len(streams), flushed=True).items():
+                ingested, split = self._resample_in(streams, [None] * len(streams), flushed=True)
+                for s, x in ingested.items():
                     if x.numel():
                         s._append(x)
+                for s, x in split.items():
+                    if x.numel():
+                        s._spread.x.append(x)
                 live = [s for s in streams if s.n_samples > 0]
                 for s in live:
                     s.n_final = -(-s.n_samples // self.hop)
@@ -505,6 +615,7 @@ class StreamGroup:
                                  flushed=True)
                 for s in streams:
                     out.setdefault(s, s._output([]))
+                out = self._spread_out(out, flushed=True)
                 out = self._resample_out(out, flushed=True)
         finally:
             # a stream is ended whether or not its last tick succeeded: a failed flush leaves no half-advanced stream
@@ -557,23 +668,49 @@ class StreamGroup:
         self.close()
 
     # ------------------------------------------------------------------ rate conversion
-    def _resample_in(self, streams, xs, flushed: bool) -> Dict[SeparationStream, torch.Tensor]:
+    def _resample_in(self, streams, xs, flushed: bool):
         """Ingest of a tick, one sab_resample call for every stream that has a resampler in front: the codec-rate
-        samples that became computable (all the rest at flush()), per stream.  xs: the pushed [C, S] (None at flush)."""
-        segs, outs = [], {}
+        samples that became computable (all the rest at flush()), per stream, as (mono [S] per stream, channels [C, S]
+        per keep-channels stream at another rate).  xs: the pushed [C, S] (None at flush)."""
+        segs, outs, split = [], {}, {}
         for s, x in zip(streams, xs):
-            r = s._ingest
-            if r is None:
-                continue
-            if x is not None:
-                r.append(x)
-            sg, out = r.take(flushed)
-            segs += sg
-            outs[s] = out[0]
+            for r, into in ((s._ingest, outs), (s._split, split)):
+                if r is None:
+                    continue
+                if x is not None:
+                    r.append(x)
+                sg, out = r.take(flushed)
+                segs += sg
+                into[s] = out[0] if r.mean else out
         self.model._ensure_engine().resample(segs)
         for s in outs:
             s._ingest.trim()
-        return outs
+        for s in split:
+            s._split.trim()
+        return outs, split
+
+    def _spread_out(self, out: Dict[SeparationStream, StreamOutput], flushed: bool) -> Dict[SeparationStream,
+                                                                                           StreamOutput]:
+        """The multichannel stage of a tick, one sab_spread_channels call for every keep-channels stream: the codec-rate
+        mono samples that became final are appended to its _Spread, and the [C, S] stems whose frames are all
+        computable (all the rest at flush(), when both lengths are known) replace them."""
+        segs, ys = [], {}
+        for s, o in out.items():
+            sp = s._spread
+            if sp is None:
+                continue
+            if o.target.numel():
+                sp.tr.append(torch.stack([o.target, o.residual]))
+            if flushed:
+                sp.tr_length, sp.x_length = sp.tr.received, sp.x.received
+            seg, ys[s] = sp.take()
+            if seg is not None:
+                segs.append(seg)
+        self.model._ensure_engine().spread_channels(segs)
+        for s, y in ys.items():
+            s._spread.trim()
+            out[s] = StreamOutput(target=y[0], residual=y[1])
+        return out
 
     def _resample_out(self, out: Dict[SeparationStream, StreamOutput], flushed: bool) -> Dict[SeparationStream,
                                                                                              StreamOutput]:
@@ -585,13 +722,14 @@ class StreamGroup:
             if r is None:
                 continue
             if o.target.numel():
-                r.append(torch.stack([o.target, o.residual]))
+                r.append(torch.cat([o.target, o.residual]) if s.keep_channels else torch.stack([o.target, o.residual]))
             sg, ys[s] = r.take(flushed)
             segs += sg
         self.model._ensure_engine().resample(segs)
         for s, y in ys.items():
             s._emit.trim()
-            out[s] = StreamOutput(target=y[0], residual=y[1])
+            h = y.shape[0] // 2                            # 1, or C with keep_channels
+            out[s] = StreamOutput(target=y[:h] if s.keep_channels else y[0], residual=y[h:] if s.keep_channels else y[1])
         return out
 
     # ------------------------------------------------------------------ the tick
@@ -831,21 +969,42 @@ class StreamGroup:
         them), then their state is released and they leave the queue."""
         sr = self.model.sample_rate
         done = [j for j in jobs if not j.done and j._dec_next == len(j._dec_tiles)]
-        segs, outs = [], []
+        spread, ys = [], []                                     # keep_channels: the stems of every channel first
         for j in done:
             y = j._out
+            if j.keep_channels:
+                C, n, S = j._x48.shape[0], y.shape[1], j._x48.shape[1]
+                y = torch.empty(2 * C, n, device=self.device, dtype=torch.float32)
+                spread.append(dict(channels=C, target=j._out[0].data_ptr(), residual=j._out[1].data_ptr(), tr_first=0,
+                                   tr_count=n, tr_length=n, mix=j._x48.data_ptr(), mix_channel_stride=S, mix_first=0,
+                                   mix_count=S, mix_length=S, out_target=y[:C].data_ptr(),
+                                   out_residual=y[C:].data_ptr(), out_channel_stride=n, out_first=0, out_count=n))
+            ys.append(y)
+        self.model._ensure_engine().spread_channels(spread)
+        segs, outs = [], []
+        for j, x in zip(done, ys):
+            y = x
             if j.sample_rate != sr:
-                n = y.shape[1]
-                y = torch.empty(2, resampled_length(n, sr, j.sample_rate), device=self.device, dtype=torch.float32)
-                segs += [dict(orig_rate=sr, new_rate=j.sample_rate, in_=j._out[r].data_ptr(), in_first=0, in_count=n,
-                              length=n, out=y[r].data_ptr(), out_first=0, out_count=y.shape[1]) for r in range(2)]
+                n = x.shape[1]
+                y = torch.empty(x.shape[0], resampled_length(n, sr, j.sample_rate), device=self.device,
+                                dtype=torch.float32)
+                segs += [dict(orig_rate=sr, new_rate=j.sample_rate, in_=x[r].data_ptr(), in_first=0, in_count=n,
+                              length=n, out=y[r].data_ptr(), out_first=0, out_count=y.shape[1]) for r in range(x.shape[0])]
             outs.append(y)
         self.model._ensure_engine().resample(segs)
         for j, y in zip(done, outs):
             j._release()
-            j._result = StreamOutput(target=y[0], residual=y[1])
+            h = y.shape[0] // 2
+            j._result = StreamOutput(target=y[:h] if j.keep_channels else y[0],
+                                     residual=y[h:] if j.keep_channels else y[1])
             j.done = True
             self._jobs.remove(j)
+
+
+def check_keep_channels(keep_channels) -> bool:
+    if not isinstance(keep_channels, bool):
+        raise TypeError(f"keep_channels must be True or False, got {keep_channels!r}")
+    return keep_channels
 
 
 def _drop_group(hold_plan_limits, key, jobs):
